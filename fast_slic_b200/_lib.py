@@ -19,7 +19,7 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_iterate_host_async", "fslic_b200_wait", "fslic_b200_create_cca",
     "fslic_b200_debug_assign_impl", "fslic_b200_connectivity_scratch_bytes", "fslic_b200_get_connectivity",
     "fslic_b200_get_mask_density", "fslic_b200_cluster_density_to_mask", "fslic_b200_cca_stage_ms",
-    "fslic_b200_iterate_real", "fslic_b200_iterate_preemptive",
+    "fslic_b200_iterate_real", "fslic_b200_iterate_preemptive", "fslic_b200_set_manhattan_spatial_dist",
 )
 
 STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity", "iterate")
@@ -65,6 +65,7 @@ def lib():
     L.fslic_b200_iterate.argtypes = [vp, vp, vp, vp, i32, C.POINTER(Params), vp]
     L.fslic_b200_iterate_real.argtypes = [vp, i32, vp, vp, vp, i32, C.POINTER(Params), vp]
     L.fslic_b200_iterate_preemptive.argtypes = [vp, vp, vp, vp, i32, C.POINTER(Params), C.c_float, vp]
+    L.fslic_b200_set_manhattan_spatial_dist.argtypes = [vp, i32]
     L.fslic_b200_iterate_host.argtypes = [vp, vp, vp, vp, i32, C.POINTER(Params)]
     L.fslic_b200_iterate_host_async.argtypes = [vp, vp, vp, vp, i32, C.POINTER(Params)]
     L.fslic_b200_wait.argtypes = [vp]

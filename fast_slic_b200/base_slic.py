@@ -3,7 +3,7 @@
 Mirrors fast-slic/fast_slic/base_slic.py:3-62 (BaseSlic / Slic: same kwargs, defaults,
 properties, return dtype) and the Cython ``SlicModel`` (fast-slic/cfast_slic.pyx:15-260,
 attributes cfast_slic.pxd:104-120).  Implemented: the default integer-distance path of the north star, the
-float-distance variants and `preemptive`; LSC raises NotImplementedError.
+float-distance variants, `preemptive` and `manhattan_spatial_dist=False`; LSC raises NotImplementedError.
 """
 import collections
 import contextlib
@@ -194,12 +194,8 @@ class SlicModel(object):
     def _unsupported(self):
         if self.real_dist and self.real_dist_type not in Engine.REAL_DIST_VARIANTS:
             raise NotImplementedError("real_dist_type %r (LSC) is outside the CUDA hot path" % (self.real_dist_type,))
-        if self.real_dist and self.real_dist_type == "noq" and not self.manhattan_spatial_dist:
-            raise NotImplementedError("SlicRealDistNoQ with manhattan_spatial_dist=False is outside the CUDA hot path")
         if self.preemptive and self.real_dist:
             raise NotImplementedError("preemptive=True together with a float-distance variant is outside the CUDA hot path")
-        if not self.manhattan_spatial_dist:
-            raise NotImplementedError("manhattan_spatial_dist=False is outside the CUDA hot path")
 
     def initialize(self, image):
         """cfast_slic.pyx:124-147."""
@@ -225,7 +221,7 @@ class SlicModel(object):
         clusters = np.ascontiguousarray(self._clusters)[None]
         # the lock covers the timing read-out too: it belongs to this call, not to another thread's next one
         with _locked(lambda: get_engine(H, W, self._num_components, 1, self.device)) as eng:
-            labels = eng.iterate_host(image[None], clusters, params)
+            labels = eng.iterate_host(image[None], clusters, params, manhattan_spatial_dist=self.manhattan_spatial_dist)
             ms = eng.stage_ms()
             cca = eng.cca_stage_ms()
         self._clusters = clusters[0]
@@ -252,10 +248,11 @@ def _iterate_real_dist(self, image, params):
         with torch.cuda.device(eng.device):
             img = torch.from_numpy(image).to(eng.device)[None]
             cl = torch.from_numpy(np.ascontiguousarray(self._clusters).view(np.uint8).reshape(1, -1, 32).copy()).to(eng.device)
+            spatial = dict(manhattan_spatial_dist=self.manhattan_spatial_dist)  # cfast_slic.pyx:186,246
             if self.preemptive:  # cfast_slic.pyx:183-184
-                labels = eng.iterate_preemptive(img, cl, params, self.preemptive_thres)
+                labels = eng.iterate_preemptive(img, cl, params, self.preemptive_thres, **spatial)
             else:
-                labels = eng.iterate_real(self.real_dist_type, img, cl, params)
+                labels = eng.iterate_real(self.real_dist_type, img, cl, params, **spatial)
             ms = eng.stage_ms()
             self._clusters = cl[0].cpu().numpy().view(CLUSTER_DTYPE).reshape(-1)
             out = labels[0].cpu().numpy()
@@ -439,6 +436,7 @@ class BaseSlic(object):
             if images.dtype != np.uint8:
                 raise ValueError("images must be uint8")
         m = self._slic_model
+        spatial = dict(manhattan_spatial_dist=m.manhattan_spatial_dist)
         with _locked(lambda: get_engine(H, W, K, B, device)) as eng:
             if m.real_dist or m.preemptive:
                 # the float-distance contexts and `preemptive` have device entry points only: host batches go up and down here
@@ -451,9 +449,9 @@ class BaseSlic(object):
                     else:
                         d_cl = torch.from_numpy(np.ascontiguousarray(clusters).view(np.uint8).reshape(B, K, 32).copy()).to(eng.device)
                     if m.preemptive:
-                        d_lab = eng.iterate_preemptive(d_img, d_cl, params, m.preemptive_thres)
+                        d_lab = eng.iterate_preemptive(d_img, d_cl, params, m.preemptive_thres, **spatial)
                     else:
-                        d_lab = eng.iterate_real(m.real_dist_type, d_img, d_cl, params)
+                        d_lab = eng.iterate_real(m.real_dist_type, d_img, d_cl, params, **spatial)
                     if is_tensor:
                         labels, clusters = d_lab, d_cl
                     else:
@@ -462,11 +460,11 @@ class BaseSlic(object):
             elif is_tensor:
                 if clusters is None:
                     clusters = eng.initialize_clusters(images)
-                labels = eng.iterate(images, clusters, params)
+                labels = eng.iterate(images, clusters, params, **spatial)
             else:
                 if clusters is None:
                     clusters = eng.initialize_clusters_host(images)
-                labels = eng.iterate_host(images, clusters, params)
+                labels = eng.iterate_host(images, clusters, params, **spatial)
         return (labels, clusters) if return_clusters else labels
 
 

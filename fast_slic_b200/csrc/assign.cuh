@@ -566,19 +566,35 @@ __global__ void __launch_bounds__(256) k_prepare2(PrepParams pp, fslic_cluster* 
 
 // ---------------------------------------------------------------------------------------------
 // Spatial patch (BaseContext::set_spatial_patch, context.cpp:23-40), laid out for LINEAR addressing:
-//   tbl[(di + OY) * TS + (dj + OX)] = (u16)(coef * (float)(|di| + |dj|))  inside the (2S+1)^2 window,
-//                                   = FSLIC_BIGSP                         outside it,
+//   tbl[(di + OY) * TS + (dj + OX)] = spatial_u16(coef, di, dj)  inside the (2S+1)^2 window,
+//                                   = FSLIC_BIGSP                outside it,
 // for di in [-OY, OY], dj in [-OX, OX].  A pixel's entry for candidate c is then at
 //   (i*TS + j) + ((OY - cy)*TS + (OX - cx)):  a per-thread constant plus a per-candidate constant,
 // so the window predicate and both abs() disappear from the inner loop.
 // ---------------------------------------------------------------------------------------------
-__global__ void k_build_sptable(uint16_t* __restrict__ tbl, int S, int OY, int OX, int TS, float coef) {
+// The spatial term of the u16 contexts: (u16)(coef * (|di| + |dj|)) with manhattan_spatial_dist (the default),
+// (u16)(coef * hypotf(di, dj)) without it (context.cpp:27-38).  The reference's hypotf is glibc's, which returns the
+// correctly rounded sqrtf(di^2 + dj^2) for every offset a context produces (|di|, |dj| <= 32767; checked exhaustively
+// by tests/test_euclidean_cpu.py).  CUDA's hypotf is not correctly rounded, so euclid_dist rounds the exact integer
+// square sum itself: a float square root is exact while the sum fits 24 bits, a double one (rounded once more to
+// float: harmless for a square root of a 31-bit integer) beyond.
+__device__ __forceinline__ float euclid_dist(int di, int dj) {
+    const int n = di * di + dj * dj;  // <= 2 * 32767^2 < 2^31
+    return n <= (1 << 24) ? __fsqrt_rn((float)n) : __double2float_rn(__dsqrt_rn((double)n));
+}
+
+__device__ __forceinline__ uint32_t spatial_u16(float coef, int di, int dj, int manhattan) {
+    const float m = manhattan ? (float)(abs(di) + abs(dj)) : euclid_dist(di, dj);
+    return (uint16_t)__float2uint_rz(__fmul_rn(coef, m));
+}
+
+__global__ void k_build_sptable(uint16_t* __restrict__ tbl, int S, int OY, int OX, int TS, float coef, int manhattan) {
     const int n = (2 * OY + 1) * TS;
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
         const int r = t / TS, c = t - r * TS;
         const int di = abs(r - OY), dj = abs(c - OX);
         uint16_t v = (uint16_t)FSLIC_BIGSP;
-        if (di <= S && dj <= S && c <= 2 * OX) v = (uint16_t)__float2uint_rz(__fmul_rn(coef, (float)(di + dj)));
+        if (di <= S && dj <= S && c <= 2 * OX) v = (uint16_t)spatial_u16(coef, di, dj, manhattan);
         tbl[t] = v;
     }
 }
@@ -595,6 +611,7 @@ struct AssignParams {
     int tiles_x, tiles_y, ntiles;  // warp tiles (32 columns x R sub-rows) per image
     int tps;           // warp tiles per super tile: AS_T, or 1 when the launch is too small to fill the GPU otherwise
     float coef;        // generic path only
+    int manhattan;     // manhattan_spatial_dist: 1 = |di| + |dj|, 0 = Euclidean (read where the term is computed inline)
     // k_assign5 only: everything warp uniform that the host can precompute lives in the constant bank, so the kernel
     // neither keeps it in registers nor re-derives it (the compiler rematerialised the divisions per super tile)
     int stx, per_img, total;        // super tiles per tile row / per image / in all
@@ -621,10 +638,13 @@ __device__ __forceinline__ void acc_add_pixel(unsigned long long* ac, uint32_t l
 
 // Brute-force assignment of one pixel straight from the cell grid: lexicographic minimum of
 // (d, phase, k) over the clusters whose window covers (i, j).  Returns the new label (or the kept
-// one) and stores it.  Used by the generic kernel and by warp tiles whose candidate list overflowed.
+// one) and stores it.  Used by the generic kernel and by warp tiles whose candidate list overflowed.  The warp-tile
+// kernels pass their spatial patch in shared memory (TS > 0: its row pitch) and read the term from it, like their main
+// loop; the generic kernel computes it.
+template <int TS = 0>
 __device__ __forceinline__ uint32_t assign_pixel_generic(const AssignParams& ap, int i, int j, uint32_t q,
                                                           const CInfo* __restrict__ ci, const int* __restrict__ cs,
-                                                          uint16_t* __restrict__ lb) {
+                                                          uint16_t* __restrict__ lb, const uint16_t* s_tbl = nullptr) {
     const int S = ap.S, W = ap.W, H = ap.H;
     unsigned long long best = ~0ull;
     const int cr0 = max(i - S, 0) / ap.G, cr1 = min(i + S, H - 1) / ap.G;
@@ -634,9 +654,10 @@ __device__ __forceinline__ uint32_t assign_pixel_generic(const AssignParams& ap,
         for (int u = s; u < e; u++) {
             const CInfo r = ci[u];
             const int cy = (int16_t)(r.cyx & 0xffff), cx = r.cyx >> 16;
-            const int di = abs(i - cy), dj = abs(j - cx);
-            if (di > S || dj > S) continue;
-            const uint32_t sp = (uint16_t)__float2uint_rz(__fmul_rn(ap.coef, (float)(di + dj)));
+            const int di = i - cy, dj = j - cx;
+            if (abs(di) > S || abs(dj) > S) continue;
+            const uint32_t sp = TS ? (uint32_t)s_tbl[(di + ap.OY) * TS + (dj + ap.OX)]
+                                   : spatial_u16(ap.coef, di, dj, ap.manhattan);
             const uint32_t d = sad4_acc(q, r.color, sp) & 0xffffu;  // u16 arithmetic like the scalar reference
             const unsigned long long key = ((unsigned long long)d << 32) | r.sortkey;
             best = key < best ? key : best;
@@ -862,7 +883,7 @@ __global__ void __launch_bounds__(AS_THREADS, AS_MINB) k_assign_warp(AssignParam
                 for (int rr = 0; rr < R; rr++) {
                     if (colok && rr < nrow) {
                         const int i = wi0 + rr * stride;
-                        const uint32_t label = assign_pixel_generic(ap, i, j, q[rr], ci, cs, labels + img_off);
+                        const uint32_t label = assign_pixel_generic<TS>(ap, i, j, q[rr], ci, cs, labels + img_off, s_tbl);
                         if (UPDATE && label != 0xFFFF) acc_add_pixel(ac, label, i, j, q[rr]);
                     }
                 }

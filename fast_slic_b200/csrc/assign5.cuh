@@ -310,7 +310,8 @@ __global__ void __launch_bounds__(32 * A5_MAXWARPS, 1)
                 for (int rr = 0; rr < R; rr++) {
                     if (j < W && rr < nrow) {
                         const int i = wi0 + rr * stride;
-                        const uint32_t label = assign_pixel_generic(ap, i, j, q[rr], ci, cs, labels + img_off);
+                        const uint32_t label = assign_pixel_generic<TS>(ap, i, j, q[rr], ci, cs, labels + img_off,
+                                                                        reinterpret_cast<const uint16_t*>(smem_raw));
                         if (UPDATE && label != 0xFFFF) acc_add_pixel(ac, label, i, j, q[rr]);
                     }
                 }

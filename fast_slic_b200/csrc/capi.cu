@@ -137,7 +137,8 @@ struct fslic_ctx {
         const void *img, *cl, *lab;
         int batch;
         fslic_params p;
-    } gkey = {nullptr, nullptr, nullptr, 0, {0.f, 0.f, 0, 0, 0, 0}}, gkey_seen = {nullptr, nullptr, nullptr, 0, {0.f, 0.f, 0, 0, 0, 0}};
+        int manhattan;
+    } gkey = {nullptr, nullptr, nullptr, 0, {0.f, 0.f, 0, 0, 0, 0}, 0}, gkey_seen = {nullptr, nullptr, nullptr, 0, {0.f, 0.f, 0, 0, 0, 0}, 0};
     int glaunches = 0;
     float assign_kernel_ms = 0.f;
     int assign_kernel_launches = 0;
@@ -145,6 +146,8 @@ struct fslic_ctx {
     int spt_stride = 0;
     cudaStream_t spt_stream = nullptr;
     uint32_t spt_coef_bits = 0;
+    int spt_manhattan = 1;
+    int manhattan = 1;         // manhattan_spatial_dist (fslic_b200_set_manhattan_spatial_dist): read by every iterate
     int assign_impl = 5;       // 5: TMA-staged kernel where it applies (default), 4: always the LDG kernel (FSLIC_ASSIGN=4)
     int last_assign_impl = 0;  // which kernel the last subsampled / full pass used (tests, bench)
 };
@@ -155,6 +158,11 @@ extern "C" int fslic_b200_sizeof_cluster(void) { return (int)sizeof(fslic_cluste
 extern "C" int fslic_b200_get_S(const fslic_ctx* ctx) { return ctx ? ctx->S : -1; }
 extern "C" int fslic_b200_launches_last_iterate(const fslic_ctx* ctx) { return ctx ? ctx->last_launches : -1; }
 extern "C" int fslic_b200_debug_assign_impl(const fslic_ctx* ctx) { return ctx ? ctx->last_assign_impl : -1; }
+extern "C" int fslic_b200_set_manhattan_spatial_dist(fslic_ctx* ctx, int on) {
+    if (!ctx) return set_err(FSLIC_EINVAL, "NULL context");
+    ctx->manhattan = on ? 1 : 0;
+    return FSLIC_OK;
+}
 
 // ---- Lab tables: FastCIELabCvt ctor, fast-slic/src/cielab.h:297-305 ----------------------
 // _srgb_gamma_tbl (cielab.h:22-279) is the sRGB inverse companding curve documented at
@@ -686,7 +694,7 @@ static bool make_subrow_map(CUtensorMap* m, CUtensorMapDataType dt, int esize, v
 }
 
 static int build_patches(fslic_ctx* c, int stride, bool need_sub, float coef, cudaStream_t st, int* launches) {
-    // The two patches depend on (S, stride, coef) only: consecutive calls with the same parameters reuse them (two
+    // The two patches depend on (S, stride, coef, manhattan) only: consecutive calls with the same parameters reuse them (two
     // launches less per call, four on the sliced host path).  Inside a stream capture they are always rebuilt, so a
     // replayed graph never depends on what an unrelated call left in the buffers.
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
@@ -694,23 +702,24 @@ static int build_patches(fslic_ctx* c, int stride, bool need_sub, float coef, cu
     uint32_t coef_bits;
     memcpy(&coef_bits, &coef, 4);
     const bool warm = cap == cudaStreamCaptureStatusNone && c->spt_valid && c->spt_stream == st && c->spt_stride == stride &&
-                      c->spt_coef_bits == coef_bits && (c->spt_has_sub || !need_sub);
+                      c->spt_coef_bits == coef_bits && c->spt_manhattan == c->manhattan && (c->spt_has_sub || !need_sub);
     if (warm) return FSLIC_OK;
     c->spt_valid = true;
     c->spt_stream = st;  // a call on another stream is not ordered after this build: it rebuilds
     c->spt_stride = stride;
     c->spt_coef_bits = coef_bits;
+    c->spt_manhattan = c->manhattan;
     c->spt_has_sub = need_sub;
     if (need_sub) {
         const PassGeom g = pass_geometry(c, stride);
         if (g.fast) {
-            k_build_sptable<<<64, 256, 0, st>>>(c->sptable, c->S, g.OY, g.OX, g.TS, coef);
+            k_build_sptable<<<64, 256, 0, st>>>(c->sptable, c->S, g.OY, g.OX, g.TS, coef, c->manhattan);
             if (launches) *launches += 1;
         }
     }
     const PassGeom gf = pass_geometry(c, 1);
     if (gf.fast) {
-        k_build_sptable<<<64, 256, 0, st>>>(c->sptable + SPT_MAX_ELEMS, c->S, gf.OY, gf.OX, gf.TS, coef);
+        k_build_sptable<<<64, 256, 0, st>>>(c->sptable + SPT_MAX_ELEMS, c->S, gf.OY, gf.OX, gf.TS, coef, c->manhattan);
         if (launches) *launches += 1;
     }
     CK(cudaGetLastError());
@@ -734,6 +743,7 @@ static int run_assign_pass(fslic_ctx* c, int batch, int stride, int rem, int cfg
         ap.cfg_stride = cfg_stride; ap.fresh_from = fresh_from;
         ap.G = c->G; ap.cellW = c->cellW; ap.cellH = c->cellH; ap.ncell = c->ncell;
         ap.coef = coef;
+        ap.manhattan = c->manhattan;
         const long px = (long)ap.nsub * c->W * batch;
         long grid = (px + 255) / 256;
         if (grid > (long)c->num_sms * 32) grid = (long)c->num_sms * 32;
@@ -757,6 +767,7 @@ static int run_assign_pass(fslic_ctx* c, int batch, int stride, int rem, int cfg
         ap.cfg_stride = cfg_stride; ap.fresh_from = fresh_from;
         ap.G = c->G; ap.cellW = c->cellW; ap.cellH = c->cellH; ap.ncell = c->ncell;
         ap.coef = coef;
+        ap.manhattan = c->manhattan;
         const long px = (long)ap.nsub * c->W * batch;
         long grid = (px + 255) / 256;
         if (grid > (long)c->num_sms * 32) grid = (long)c->num_sms * 32;
@@ -787,6 +798,7 @@ static int run_assign_pass(fslic_ctx* c, int batch, int stride, int rem, int cfg
     ap.tiles_y = ceil_div(ap.nsub, g.R);
     ap.ntiles = ap.tiles_x * ap.tiles_y;
     ap.coef = coef;
+    ap.manhattan = c->manhattan;  // the warp-tile kernels read the patch built with it; k_assign_generic reads it
     ap.tps = AS_T;
     ap.fuse_prepare = 0;
     // The TMA-staged kernel: row strides of the tensor maps must be multiples of 16 bytes (W % 8 == 0 for the u16
@@ -1105,7 +1117,7 @@ extern "C" int fslic_b200_iterate(fslic_ctx* c, const uint8_t* d_images, fslic_c
     if (c && p && c->graphs_enabled && batch > 0 && batch < 4 && p->collect_timing == 0 && stream != nullptr) {
         fslic_ctx::GraphKey k;
         memset(&k, 0, sizeof(k));
-        k.img = nullptr; k.cl = d_clusters; k.lab = d_labels; k.batch = batch; k.p = *p;
+        k.img = nullptr; k.cl = d_clusters; k.lab = d_labels; k.batch = batch; k.p = *p; k.manhattan = c->manhattan;
         const bool have = c->gexec && memcmp(&k, &c->gkey, sizeof(k)) == 0;
         const bool again = memcmp(&k, &c->gkey_seen, sizeof(k)) == 0;
         memcpy(&c->gkey_seen, &k, sizeof(k));
@@ -1115,7 +1127,7 @@ extern "C" int fslic_b200_iterate(fslic_ctx* c, const uint8_t* d_images, fslic_c
 }
 
 // The float-distance contexts of the reference (context.h:100-125; cfast_slic.pyx:198-252): variant 0 = ContextRealDist
-// ("standard"), 1 = ContextRealDistL2, 2 = ContextRealDistNoQ with manhattan_spatial_dist (its default).
+// ("standard"), 1 = ContextRealDistL2, 2 = ContextRealDistNoQ; c->manhattan selects the spatial term of variants 0 and 2.
 extern "C" int fslic_b200_iterate_real(fslic_ctx* c, int variant, const uint8_t* d_images, fslic_cluster* d_clusters,
                                        uint16_t* d_labels, int batch, const fslic_params* p, void* stream) {
     if (variant < 0 || variant > 2) return set_err(FSLIC_EINVAL, "variant must be 0 (standard), 1 (l2) or 2 (noq)");
@@ -1242,15 +1254,18 @@ static int iterate_graphed(fslic_ctx* c, const uint8_t* d_images, fslic_cluster*
     if (rc) return rc;
     fslic_ctx::GraphKey k;
     memset(&k, 0, sizeof(k));
-    k.img = nullptr; k.cl = d_clusters; k.lab = d_labels; k.batch = batch; k.p = *p;
+    k.img = nullptr; k.cl = d_clusters; k.lab = d_labels; k.batch = batch; k.p = *p; k.manhattan = c->manhattan;
     {
         USE_DEVICE(c->device);
         c->slice = 0;
         rc = launch_lab(c, d_images, c->quad, batch, p->convert_to_lab, st);
         if (rc) return rc;
     }
+    // A replay rebuilds the spatial patches for the graph's parameters behind the cache's back (build_patches keeps
+    // what the last plain build left), so after any graph launch the next plain call must rebuild them.
     if (c->gexec && memcmp(&k, &c->gkey, sizeof(k)) == 0) {
         CK(cudaGraphLaunch(c->gexec, st));
+        c->spt_valid = false;
         c->last_launches = c->glaunches;
         return FSLIC_OK;
     }
@@ -1281,6 +1296,7 @@ static int iterate_graphed(fslic_ctx* c, const uint8_t* d_images, fslic_cluster*
     memcpy(&c->gkey, &k, sizeof(k));
     c->glaunches = c->last_launches;
     CK(cudaGraphLaunch(c->gexec, st));
+    c->spt_valid = false;
     return FSLIC_OK;
 }
 

@@ -71,6 +71,10 @@ class Engine:
         if images.shape[0] > self.max_batch:
             raise ValueError("batch larger than the engine's max_batch")
 
+    def _set_spatial(self, manhattan_spatial_dist):
+        """The context's manhattan_spatial_dist for the next enqueue (call with `lock` held)."""
+        check(self._L.fslic_b200_set_manhattan_spatial_dist(self._h, int(bool(manhattan_spatial_dist))))
+
     def new_clusters(self, batch):
         return torch.zeros((batch, self.K, 32), dtype=torch.uint8, device=self.device)
 
@@ -91,38 +95,42 @@ class Engine:
                                                          _stream_ptr(self.device)))
         return clusters
 
-    def iterate(self, images, clusters, params, labels=None):
-        """images u8[B,H,W,3] (cuda), clusters u8[B,K,32] (cuda, updated in place) -> labels u16 as int16[B,H,W]."""
+    def iterate(self, images, clusters, params, labels=None, manhattan_spatial_dist=True):
+        """images u8[B,H,W,3] (cuda), clusters u8[B,K,32] (cuda, updated in place) -> labels u16 as int16[B,H,W].
+        manhattan_spatial_dist=False: Euclidean spatial distance (every iterate entry point takes it)."""
         self._check_images(images)
         B = images.shape[0]
         if labels is None:
             labels = torch.empty((B, self.H, self.W), dtype=torch.int16, device=self.device)
         with self.lock:
+            self._set_spatial(manhattan_spatial_dist)
             check(self._L.fslic_b200_iterate(self._h, images.data_ptr(), clusters.data_ptr(), labels.data_ptr(), B,
                                              C.byref(params), _stream_ptr(self.device)))
         return labels
 
     REAL_DIST_VARIANTS = {"standard": 0, "l2": 1, "noq": 2}
 
-    def iterate_real(self, variant, images, clusters, params, labels=None):
+    def iterate_real(self, variant, images, clusters, params, labels=None, manhattan_spatial_dist=True):
         """Float-distance variants (fslic_b200_iterate_real): variant "standard" | "l2" | "noq"; device tensors."""
         self._check_images(images)
         B = images.shape[0]
         if labels is None:
             labels = torch.empty((B, self.H, self.W), dtype=torch.int16, device=self.device)
         with self.lock:
+            self._set_spatial(manhattan_spatial_dist)
             check(self._L.fslic_b200_iterate_real(self._h, self.REAL_DIST_VARIANTS[variant], images.data_ptr(),
                                                   clusters.data_ptr(), labels.data_ptr(), B, C.byref(params),
                                                   _stream_ptr(self.device)))
         return labels
 
-    def iterate_preemptive(self, images, clusters, params, preemptive_thres, labels=None):
+    def iterate_preemptive(self, images, clusters, params, preemptive_thres, labels=None, manhattan_spatial_dist=True):
         """`preemptive=True` of the reference (fslic_b200_iterate_preemptive); device tensors like iterate()."""
         self._check_images(images)
         B = images.shape[0]
         if labels is None:
             labels = torch.empty((B, self.H, self.W), dtype=torch.int16, device=self.device)
         with self.lock:
+            self._set_spatial(manhattan_spatial_dist)
             check(self._L.fslic_b200_iterate_preemptive(self._h, images.data_ptr(), clusters.data_ptr(), labels.data_ptr(), B,
                                                         C.byref(params), C.c_float(preemptive_thres), _stream_ptr(self.device)))
         return labels
@@ -165,19 +173,21 @@ class Engine:
             check(self._L.fslic_b200_initialize_clusters_host(self._h, images_np.ctypes.data, clusters.ctypes.data, B))
         return clusters
 
-    def iterate_host(self, images_np, clusters_np, params, labels_np=None):
+    def iterate_host(self, images_np, clusters_np, params, labels_np=None, manhattan_spatial_dist=True):
         B = images_np.shape[0]
         if labels_np is None:
             labels_np = np.empty((B, self.H, self.W), np.int16)
         with self.lock:
+            self._set_spatial(manhattan_spatial_dist)
             check(self._L.fslic_b200_iterate_host(self._h, images_np.ctypes.data, clusters_np.ctypes.data,
                                                   labels_np.ctypes.data, B, C.byref(params)))
         return labels_np
 
-    def iterate_host_async(self, images_np, clusters_np, params, labels_np):
+    def iterate_host_async(self, images_np, clusters_np, params, labels_np, manhattan_spatial_dist=True):
         """Enqueue one host batch and return; `wait()` blocks until labels_np / clusters_np are filled.
         All three arrays must live in pinned memory and must not be touched in between."""
         self._inflight = (images_np, clusters_np, labels_np, params)  # keep the buffers alive
+        self._set_spatial(manhattan_spatial_dist)
         check(self._L.fslic_b200_iterate_host_async(self._h, images_np.ctypes.data, clusters_np.ctypes.data,
                                                     labels_np.ctypes.data, images_np.shape[0], C.byref(params)))
 

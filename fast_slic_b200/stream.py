@@ -34,7 +34,8 @@ class _Slot:
 
 class SlicStream:
     def __init__(self, height, width, num_components, batch, depth=2, device=0, compactness=10.0,
-                 min_size_factor=0.25, subsample_stride=3, convert_to_lab=True, max_iter=10, warm_start=False):
+                 min_size_factor=0.25, subsample_stride=3, convert_to_lab=True, max_iter=10, warm_start=False,
+                 manhattan_spatial_dist=True):
         require_cuda()
         if depth < 1:
             raise ValueError("depth must be >= 1")
@@ -47,6 +48,7 @@ class SlicStream:
         self._finished = collections.deque()   # warm start: batches a later submit had to wait for, not collected yet
         self._pristine = None  # grid seeding: depends on (H, W, K) only; colours are re-read from the image in pass 0
         self.warm_start = bool(warm_start)
+        self.manhattan_spatial_dist = bool(manhattan_spatial_dist)
         self._carry = None     # warm start: the clusters the previous batch ended with, [n, K, 32] bytes
 
     def pinned_images(self, n=None):
@@ -83,7 +85,8 @@ class SlicStream:
                 m = min(n, self._carry.shape[0])
                 cl[:m] = self._carry[:m]
         slot.n = n
-        slot.engine.iterate_host_async(images, cl, self._params, slot.labels.numpy()[:n])
+        slot.engine.iterate_host_async(images, cl, self._params, slot.labels.numpy()[:n],
+                                       manhattan_spatial_dist=self.manhattan_spatial_dist)
         self._busy.append(slot)
 
     def _collect_one(self, copy):

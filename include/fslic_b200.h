@@ -89,11 +89,17 @@ int fslic_b200_initialize_clusters(fslic_ctx* ctx, const uint8_t* d_images, fsli
 int fslic_b200_iterate(fslic_ctx* ctx, const uint8_t* d_images, fslic_cluster* d_clusters, uint16_t* d_labels,
                        int batch, const fslic_params* params, void* stream);
 
+/* == the public field BaseContext::manhattan_spatial_dist (context.h:35; cfast_slic.pyx:186,246): on (1, the default)
+ *    the spatial term is coef * (|di| + |dj|), off (0) it is coef * hypot(di, dj) (context.cpp:23-40), and the "noq"
+ *    float variant sums squares instead of absolute values (context.cpp:462-496).  The window stays (2S+1)^2 and the
+ *    "l2" variant ignores it, as in the reference.  Every iterate entry point reads the setting when it enqueues work. */
+int fslic_b200_set_manhattan_spatial_dist(fslic_ctx* ctx, int on);
+
 /* == the float-distance contexts ContextRealDist / ContextRealDistL2 / ContextRealDistNoQ (context.h:100-125,
  *    context.cpp:394-499; selected in cfast_slic.pyx:198-252 by SlicModel.real_dist_type): `variant` 0 = "standard"
  *    (the default kernel with float distances and an untruncated float spatial term), 1 = "l2" (squared colour and
- *    spatial distances), 2 = "noq" (float centroids, no quantisation in the update; Manhattan spatial term, the
- *    reference's default).  Same buffers and semantics as fslic_b200_iterate; results bit-identical to the reference
+ *    spatial distances), 2 = "noq" (float centroids, no quantisation in the update; absolute or, with
+ *    fslic_b200_set_manhattan_spatial_dist(ctx, 0), squared differences).  Same buffers and semantics as fslic_b200_iterate; results bit-identical to the reference
  *    (every float operation in its order and rounding). */
 int fslic_b200_iterate_real(fslic_ctx* ctx, int variant, const uint8_t* d_images, fslic_cluster* d_clusters,
                             uint16_t* d_labels, int batch, const fslic_params* params, void* stream);
