@@ -20,9 +20,11 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_debug_assign_impl", "fslic_b200_connectivity_scratch_bytes", "fslic_b200_get_connectivity",
     "fslic_b200_get_mask_density", "fslic_b200_cluster_density_to_mask", "fslic_b200_cca_stage_ms",
     "fslic_b200_iterate_real", "fslic_b200_iterate_preemptive", "fslic_b200_set_manhattan_spatial_dist",
+    "fslic_b200_iterate_lsc", "fslic_b200_debug_lsc_stages",
 )
 
 STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity", "iterate")
+LSC_STAGE_NAMES = ("before_iteration", "after_update")  # FSLIC_T_BEFORE_ITERATION, FSLIC_T_AFTER_UPDATE
 CCA_STAGE_NAMES = ("build_disjoint_set", "flatten", "threshold_by_area", "sort", "substitute", "output")  # cca.cpp:194-263
 
 
@@ -66,6 +68,8 @@ def lib():
     L.fslic_b200_iterate_real.argtypes = [vp, i32, vp, vp, vp, i32, C.POINTER(Params), vp]
     L.fslic_b200_iterate_preemptive.argtypes = [vp, vp, vp, vp, i32, C.POINTER(Params), C.c_float, vp]
     L.fslic_b200_set_manhattan_spatial_dist.argtypes = [vp, i32]
+    L.fslic_b200_iterate_lsc.argtypes = [vp, vp, vp, vp, i32, C.POINTER(Params), vp]
+    L.fslic_b200_debug_lsc_stages.argtypes = [vp, vp, vp, vp, i32, vp]
     L.fslic_b200_iterate_host.argtypes = [vp, vp, vp, vp, i32, C.POINTER(Params)]
     L.fslic_b200_iterate_host_async.argtypes = [vp, vp, vp, vp, i32, C.POINTER(Params)]
     L.fslic_b200_wait.argtypes = [vp]

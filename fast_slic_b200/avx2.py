@@ -9,4 +9,11 @@ class SlicAvx2(Slic):
 
 
 class LSCAvx2(LSC):
-    """== fast_slic.avx2.LSCAvx2 (avx2.py:13-14): iterate() raises NotImplementedError like LSC."""
+    """== fast_slic.avx2.LSCAvx2 (avx2.py:13-14).  iterate() raises NotImplementedError: the reference's AVX2 LSC context
+    normalises with _mm256_rcp_ps (arch/x64/avx2.h), an approximate reciprocal whose bits differ between CPU vendors,
+    so there is no single result to reproduce.  LSC(num_threads=1) is the defined one."""
+
+    def make_slic_model(self, num_components):
+        model = super(LSCAvx2, self).make_slic_model(num_components)
+        model.lsc_arch = "x64/avx2"
+        return model

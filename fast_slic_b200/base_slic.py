@@ -3,7 +3,7 @@
 Mirrors fast-slic/fast_slic/base_slic.py:3-62 (BaseSlic / Slic: same kwargs, defaults,
 properties, return dtype) and the Cython ``SlicModel`` (fast-slic/cfast_slic.pyx:15-260,
 attributes cfast_slic.pxd:104-120).  Implemented: the default integer-distance path of the north star, the
-float-distance variants, `preemptive` and `manhattan_spatial_dist=False`; LSC raises NotImplementedError.
+float-distance variants, `preemptive`, `manhattan_spatial_dist=False` and LSC with num_threads=1.
 """
 import collections
 import contextlib
@@ -128,6 +128,7 @@ class SlicModel(object):
         self.preemptive = False
         self.preemptive_thres = 0.05
         self.manhattan_spatial_dist = True
+        self.lsc_arch = "standard"  # which reference context an LSC model stands for (LSCAvx2: "x64/avx2")
         self.last_timing_report = None
         self.last_recorder_report = None
         self.device = 0
@@ -192,8 +193,18 @@ class SlicModel(object):
         return self._clusters
 
     def _unsupported(self):
-        if self.real_dist and self.real_dist_type not in Engine.REAL_DIST_VARIANTS:
-            raise NotImplementedError("real_dist_type %r (LSC) is outside the CUDA hot path" % (self.real_dist_type,))
+        if self.real_dist and self.real_dist_type == "lsc":
+            if self.lsc_arch != "standard":
+                raise NotImplementedError(
+                    "LSCAvx2 has no defined result to reproduce: the reference's AVX2 LSC context normalises with "
+                    "_mm256_rcp_ps, an approximate reciprocal whose bits differ between CPU vendors; use LSC(num_threads=1)")
+            if self.num_threads != 1:
+                raise NotImplementedError(
+                    "LSC with num_threads=%r: the reference's LSC merges per-thread partial centroid sums in whatever "
+                    "order its threads arrive, so only a single-threaded run has a defined result; pass num_threads=1"
+                    % (self.num_threads,))
+        elif self.real_dist and self.real_dist_type not in Engine.REAL_DIST_VARIANTS:
+            raise NotImplementedError("real_dist_type %r is outside the CUDA hot path" % (self.real_dist_type,))
         if self.preemptive and self.real_dist:
             raise NotImplementedError("preemptive=True together with a float-distance variant is outside the CUDA hot path")
 
@@ -241,8 +252,8 @@ class SlicModel(object):
 
 
 def _iterate_real_dist(self, image, params):
-    """cfast_slic.pyx:198-252: the float-distance contexts (fslic_b200_iterate_real) and the `preemptive` option
-    (fslic_b200_iterate_preemptive), both through device buffers."""
+    """cfast_slic.pyx:198-252: the float-distance contexts (fslic_b200_iterate_real), LSC (fslic_b200_iterate_lsc) and
+    the `preemptive` option (fslic_b200_iterate_preemptive), all through device buffers."""
     H, W, _ = image.shape
     with _locked(lambda: get_engine(H, W, self._num_components, 1, self.device)) as eng:
         with torch.cuda.device(eng.device):
@@ -251,15 +262,22 @@ def _iterate_real_dist(self, image, params):
             spatial = dict(manhattan_spatial_dist=self.manhattan_spatial_dist)  # cfast_slic.pyx:186,246
             if self.preemptive:  # cfast_slic.pyx:183-184
                 labels = eng.iterate_preemptive(img, cl, params, self.preemptive_thres, **spatial)
+            elif self.real_dist_type == "lsc":  # cfast_slic.pyx:207-214
+                labels = eng.iterate_lsc(img, cl, params, **spatial)
             else:
                 labels = eng.iterate_real(self.real_dist_type, img, cl, params, **spatial)
             ms = eng.stage_ms()
+            ms.update(eng.lsc_stage_ms())
             self._clusters = cl[0].cpu().numpy().view(CLUSTER_DTYPE).reshape(-1)
             out = labels[0].cpu().numpy()
+    # the reference's fstimer tree (context.cpp:112-192); LSC adds its two hooks in their places (:152, :170)
+    names = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity")
+    if self.real_dist_type == "lsc" and not self.preemptive:
+        names = ("cielab_conversion", "before_iteration", "assign", "update", "after_update", "full_assign",
+                 "enforce_connectivity")
     self.last_timing_report = json.dumps({
         "name": "iterate", "duration": int(ms["iterate"] * 1000),
-        "children": [{"name": n, "duration": int(ms[n] * 1000), "children": []}
-                     for n in ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity")]})
+        "children": [{"name": n, "duration": int(ms[n] * 1000), "children": []} for n in names]})
     self.last_recorder_report = b'{"snapshots":[]}'
     return out
 
@@ -439,7 +457,8 @@ class BaseSlic(object):
         spatial = dict(manhattan_spatial_dist=m.manhattan_spatial_dist)
         with _locked(lambda: get_engine(H, W, K, B, device)) as eng:
             if m.real_dist or m.preemptive:
-                # the float-distance contexts and `preemptive` have device entry points only: host batches go up and down here
+                # the float-distance contexts, LSC and `preemptive` have device entry points only: host batches go up and
+                # down here
                 with torch.cuda.device(eng.device):
                     d_img = images if is_tensor else torch.from_numpy(images).to(eng.device)
                     if clusters is None:
@@ -450,6 +469,8 @@ class BaseSlic(object):
                         d_cl = torch.from_numpy(np.ascontiguousarray(clusters).view(np.uint8).reshape(B, K, 32).copy()).to(eng.device)
                     if m.preemptive:
                         d_lab = eng.iterate_preemptive(d_img, d_cl, params, m.preemptive_thres, **spatial)
+                    elif m.real_dist_type == "lsc":
+                        d_lab = eng.iterate_lsc(d_img, d_cl, params, **spatial)
                     else:
                         d_lab = eng.iterate_real(m.real_dist_type, d_img, d_cl, params, **spatial)
                     if is_tensor:
@@ -504,8 +525,14 @@ class SlicRealDistNoQ(SlicRealDist):
 
 
 class LSC(SlicRealDist):
-    """== fast_slic.base_slic.LSC (base_slic.py:87-89), kept so that `from fast_slic import LSC` keeps importing: linear
-    spectral clustering is a different algorithm (src/lsc.cpp) outside this engine -- iterate() raises NotImplementedError."""
+    """== fast_slic.base_slic.LSC (base_slic.py:87-89): linear spectral clustering (src/lsc.cpp) on the GPU.
+
+    Ten features per pixel -- L, a, b and x, y each mapped onto a quarter circle --, weighted by their image means; the
+    assignment minimises the squared 10-D distance over the (2S+1)^2 window and the centroids are weighted 10-D means.
+    Bit-identical to the reference's ContextLSC run with num_threads=1.  That is the only thread count at which the
+    reference's result is defined (it merges per-thread partial sums in arrival order), so any other num_threads --
+    including the default -1 -- raises NotImplementedError: pass num_threads=1.  manhattan_spatial_dist is accepted and
+    has no effect; preemptive=True is refused."""
     real_dist_type = "lsc"
 
 

@@ -16,6 +16,7 @@
 #include "assign5.cuh"
 #include "graph.cuh"
 #include "realdist.cuh"
+#include "lsc.cuh"
 #include "preempt.cuh"
 #include "cca.cuh"
 #include "common.cuh"
@@ -121,7 +122,7 @@ struct fslic_ctx {
     cudaEvent_t cev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     float cca_ms[6] = {0, 0, 0, 0, 0, 0};
     bool cca_timing = false, cca_timed = false;
-    float stage_ms[FSLIC_T_COUNT] = {0, 0, 0, 0, 0, 0};
+    float stage_ms[FSLIC_T_COUNT] = {0, 0, 0, 0, 0, 0, 0, 0};
     int last_launches = 0;
     int slice = 0;  // first image of the batch slice the front half (Lab + passes) currently works on
     int max_smem_optin = 0;
@@ -148,6 +149,19 @@ struct fslic_ctx {
     uint32_t spt_coef_bits = 0;
     int spt_manhattan = 1;
     int manhattan = 1;         // manhattan_spatial_dist (fslic_b200_set_manhattan_spatial_dist): read by every iterate
+    // LSC (lsc.cuh), allocated at the first fslic_b200_iterate_lsc call
+    float* lsc_feat = nullptr;      // [B][10][N] normalised features
+    float* lsc_w = nullptr;         // [B][N]     pixel weights
+    float* lsc_tab = nullptr;       // [1024 + 2W + 2H] feature tables (lsc.cuh)
+    float* lsc_means = nullptr;     // [B][10]    feature means
+    float* lsc_cf = nullptr;        // [B][K][LSC_CF] centroid features
+    float* lsc_cf_init = nullptr;   // [B][K][10] centroid features after before_iteration (debug read-out)
+    LscBox* lsc_box = nullptr;      // [B][K]     label bounding boxes of the current pass
+    std::vector<float> lsc_htab;    // host copy of lsc_tab and the compactness it was built for
+    uint32_t lsc_tab_key = 0;
+    bool lsc_tab_valid = false;
+    std::vector<cudaEvent_t> lev;   // start / end events of each after_update launch (collect_timing)
+    int lev_used = 0;
     int assign_impl = 5;       // 5: TMA-staged kernel where it applies (default), 4: always the LDG kernel (FSLIC_ASSIGN=4)
     int last_assign_impl = 0;  // which kernel the last subsampled / full pass used (tests, bench)
 };
@@ -223,6 +237,10 @@ extern "C" int fslic_b200_destroy(fslic_ctx* c) {
     if (c->pre_cellmap) cudaFree(c->pre_cellmap);
     if (c->pre_nactive) cudaFree(c->pre_nactive);
     for (auto& e : c->pipe_ev) cudaEventDestroy(e);
+    for (void* p : {(void*)c->lsc_feat, (void*)c->lsc_w, (void*)c->lsc_tab, (void*)c->lsc_means, (void*)c->lsc_cf,
+                    (void*)c->lsc_cf_init, (void*)c->lsc_box})
+        if (p) cudaFree(p);
+    for (auto& e : c->lev) cudaEventDestroy(e);
     delete c;
     return FSLIC_OK;
 }
@@ -757,6 +775,29 @@ static int run_assign_pass(fslic_ctx* c, int batch, int stride, int rem, int cfg
         return FSLIC_OK;
     }
     if (variant == 3) variant = -1;
+    if (variant == 4) {  // LSC (lsc.cuh): one thread per pixel over the cell grid
+        AssignParams ap;
+        memset(&ap, 0, sizeof(ap));
+        ap.H = c->H; ap.W = c->W; ap.K = c->K; ap.S = c->S; ap.B = batch;
+        ap.stride = stride; ap.rem = rem;
+        ap.nsub = (c->H - rem + stride - 1) / stride;
+        if (ap.nsub <= 0) return FSLIC_OK;
+        ap.cfg_stride = cfg_stride; ap.fresh_from = fresh_from;
+        ap.G = c->G; ap.cellW = c->cellW; ap.cellH = c->cellH; ap.ncell = c->ncell;
+        const long px = (long)ap.nsub * c->W * batch;
+        long grid = (px + 255) / 256;
+        if (grid > (long)c->num_sms * 32) grid = (long)c->num_sms * 32;
+        if (update)
+            k_assign_lsc<true><<<(int)grid, 256, 0, st>>>(ap, SL_QUAD(c), SL_LABELS(c), SL_CINFO(c), SL_CELLS(c), c->lsc_feat,
+                                                          c->lsc_cf, SL_ACC(c), c->lsc_box);
+        else
+            k_assign_lsc<false><<<(int)grid, 256, 0, st>>>(ap, SL_QUAD(c), SL_LABELS(c), SL_CINFO(c), SL_CELLS(c), c->lsc_feat,
+                                                           c->lsc_cf, SL_ACC(c), c->lsc_box);
+        c->last_assign_impl = 0;
+        if (launches) *launches += 1;
+        CK(cudaGetLastError());
+        return FSLIC_OK;
+    }
     if (variant >= 0) {  // float-distance variants (realdist.cuh): one thread per pixel over the cell grid
         AssignParams ap;
         memset(&ap, 0, sizeof(ap));
@@ -1002,6 +1043,107 @@ static int check_params(const fslic_ctx* c, const fslic_params* p, float* coef_o
     return FSLIC_OK;
 }
 
+// ---- LSC (lsc.cuh) -----------------------------------------------------------------------------------------------
+// The feature tables of ContextLSC::map_image_into_feature_space (lsc.cpp:25-28, 69-101), computed with the libm calls
+// of the reference's object code: glibc's double sincos of a float angle (GCC merges each sin / cos pair into one call);
+// the colour tables round the cosine / sine to float and multiply in float, the others multiply in double.  Bit-identical
+// to the reference's as long as this machine's glibc computes the same double sin / cos (DESIGN.md section 4.9).
+static void build_lsc_tables(int H, int W, int S, float compactness, std::vector<float>& tab) {
+    tab.assign(LSC_TAB_FIXED + 2 * (size_t)W + 2 * (size_t)H, 0.f);
+    const float PI = (float)3.1415926;
+    const float halfPI = PI / 2;
+    const float ratio = compactness / 100.0f;
+    const float C_color = 20.0f;  // lsc.h:8
+    const float C_spatial = C_color * ratio;
+    double s, co;
+    for (int X = 0; X < 256; X++) {
+        const float theta = halfPI * ((float)X / 255.0f);
+        sincos((double)theta, &s, &co);
+        const float cosine = (float)co, sine = (float)s;
+        tab[512 + X] = C_color * cosine * 2.55f;
+        tab[768 + X] = C_color * sine * 2.55f;
+        tab[X] = (float)((double)C_color * co);
+        tab[256 + X] = (float)((double)C_color * s);
+    }
+    const float step = halfPI / (float)S;
+    for (int j = 0; j < W; j++) {
+        sincos((double)((float)j * step), &s, &co);
+        tab[LSC_TAB_FIXED + j] = (float)((double)C_spatial * co);
+        tab[LSC_TAB_FIXED + W + j] = (float)((double)C_spatial * s);
+    }
+    for (int i = 0; i < H; i++) {
+        sincos((double)((float)i * step), &s, &co);
+        tab[LSC_TAB_FIXED + 2 * W + i] = (float)((double)C_spatial * co);
+        tab[LSC_TAB_FIXED + 2 * W + H + i] = (float)((double)C_spatial * s);
+    }
+}
+
+static int ensure_lsc(fslic_ctx* c) {
+    if (c->lsc_feat) return FSLIC_OK;
+    const size_t B = (size_t)c->maxB, N = (size_t)c->N, K = (size_t)c->K;
+    float *feat = nullptr, *w = nullptr, *tab = nullptr, *means = nullptr, *cf = nullptr, *cfi = nullptr;
+    LscBox* box = nullptr;
+    if (dalloc(&feat, B * LSC_NF * N) != cudaSuccess || dalloc(&w, B * N) != cudaSuccess ||
+        dalloc(&tab, LSC_TAB_FIXED + 2 * (size_t)c->W + 2 * (size_t)c->H) != cudaSuccess ||
+        dalloc(&means, B * LSC_NF) != cudaSuccess || dalloc(&cf, B * K * LSC_CF) != cudaSuccess ||
+        dalloc(&cfi, B * K * LSC_NF) != cudaSuccess || dalloc(&box, B * K) != cudaSuccess) {
+        for (void* p : {(void*)feat, (void*)w, (void*)tab, (void*)means, (void*)cf, (void*)cfi, (void*)box})
+            if (p) cudaFree(p);
+        cudaGetLastError();
+        return set_err(FSLIC_ENOMEM, "out of device memory (LSC scratch)");
+    }
+    c->lsc_feat = feat; c->lsc_w = w; c->lsc_tab = tab; c->lsc_means = means; c->lsc_cf = cf; c->lsc_cf_init = cfi;
+    c->lsc_box = box;
+    c->lsc_tab_valid = false;
+    return FSLIC_OK;
+}
+
+// before_iteration (lsc.cpp:12-15): tables, feature means, weights and normalised features, initial centroid features.
+// Runs after the Lab kernel and before the first prepare, which clamps the centres (context.cpp:209-212) that
+// map_centroids_into_feature_space reads unclamped.
+static int lsc_before_iteration(fslic_ctx* c, const fslic_cluster* d_clusters, int batch, const fslic_params* p,
+                                cudaStream_t st, int* launches) {
+    uint32_t key;
+    memcpy(&key, &p->compactness, 4);
+    if (!c->lsc_tab_valid || key != c->lsc_tab_key) {
+        build_lsc_tables(c->H, c->W, c->S, p->compactness, c->lsc_htab);
+        // pageable source: the copy is staged before cudaMemcpyAsync returns, so the vector may change afterwards
+        CK(cudaMemcpyAsync(c->lsc_tab, c->lsc_htab.data(), c->lsc_htab.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+        c->lsc_tab_key = key;
+        c->lsc_tab_valid = true;
+    }
+    k_lsc_means<<<batch * LSC_NF, 32, 0, st>>>(SL_QUAD(c), c->lsc_tab, c->H, c->W, c->lsc_means);
+    const long px = (long)c->N * batch;
+    long grid = (px + 255) / 256;
+    if (grid > (long)c->num_sms * 32) grid = (long)c->num_sms * 32;
+    k_lsc_features<<<(int)grid, 256, 0, st>>>(SL_QUAD(c), c->lsc_tab, c->H, c->W, batch, c->lsc_means, c->lsc_feat, c->lsc_w);
+    k_lsc_centroids<<<ceil_div(batch * c->K, 256), 256, 0, st>>>(c->lsc_feat, c->H, c->W, c->K, c->S, batch, d_clusters,
+                                                                 c->lsc_cf, c->lsc_cf_init, c->lsc_box);
+    if (launches) *launches += 3;
+    CK(cudaGetLastError());
+    return FSLIC_OK;
+}
+
+// after_update (lsc.cpp:226-307) of the pass just assigned; timed launch by launch when collect_timing is on.
+static int lsc_after_update(fslic_ctx* c, int batch, int stride, cudaStream_t st, int* launches, bool timing) {
+    cudaEvent_t e1 = nullptr;
+    if (timing) {
+        while ((int)c->lev.size() < c->lev_used + 2) {
+            cudaEvent_t e;
+            CK(cudaEventCreate(&e));
+            c->lev.push_back(e);
+        }
+        CK(cudaEventRecord(c->lev[c->lev_used++], st));
+        e1 = c->lev[c->lev_used++];
+    }
+    k_lsc_after_update<<<ceil_div(batch * c->K, LSC_AU_WARPS), LSC_AU_WARPS * 32, 0, st>>>(
+        c->H, c->W, c->K, batch, stride, SL_LABELS(c), c->lsc_feat, c->lsc_w, c->lsc_cf, c->lsc_box);
+    if (e1) CK(cudaEventRecord(e1, st));
+    if (launches) *launches += 1;
+    CK(cudaGetLastError());
+    return FSLIC_OK;
+}
+
 // Front half of iterate (context.cpp:114-181): Lab LUT, max_iter x (assign + update), full assign, for the
 // `batch` images starting at image `b0` of the context's buffers.  Leaves the pre-CCA labels in c->labels.
 static int iterate_front(fslic_ctx* c, int b0, const uint8_t* d_images, fslic_cluster* d_clusters, int batch,
@@ -1013,6 +1155,11 @@ static int iterate_front(fslic_ctx* c, int b0, const uint8_t* d_images, fslic_cl
     if (rc) return rc;
     (*launches)++;
     if (timing) CK(cudaEventRecord(c->ev[1], st));
+    if (variant == 4) {  // LSC: before_iteration (context.cpp:151-154)
+        rc = lsc_before_iteration(c, d_clusters, batch, p, st, launches);
+        if (rc) return rc;
+        if (timing) CK(cudaEventRecord(c->ev[5], st));
+    }
     const int stride = p->subsample_stride;
     const int noq = variant == 2 ? 1 : 0;
     const int preempt = variant == 3 ? 1 : 0;
@@ -1031,6 +1178,10 @@ static int iterate_front(fslic_ctx* c, int b0, const uint8_t* d_images, fslic_cl
         rc = run_assign_pass(c, batch, stride, rem, stride, it, true, coef, st, launches, variant, cl,
                              variant < 0 ? d_clusters : nullptr, &prepared);
         if (rc) return rc;
+        if (variant == 4) {  // LSC: after_update (context.cpp:169-172); its Cluster update is the next prepare's
+            rc = lsc_after_update(c, batch, stride, st, launches, timing);
+            if (rc) return rc;
+        }
         rem = (rem + 1) % stride;
     }
     if (timing) CK(cudaEventRecord(c->ev[2], st));
@@ -1067,6 +1218,7 @@ static int iterate_plain(fslic_ctx* c, const uint8_t* d_images, fslic_cluster* d
     const bool timing = p->collect_timing != 0;
     c->kev_on = p->collect_timing >= 2;
     c->kev_used = 0;
+    c->lev_used = 0;
     c->cca_timing = timing;
     c->cca_timed = false;
     if (timing) CK(cudaEventRecord(c->ev[0], st));
@@ -1082,6 +1234,17 @@ static int iterate_plain(fslic_ctx* c, const uint8_t* d_images, fslic_cluster* d
         CK(cudaEventElapsedTime(&ms, c->ev[0], c->ev[1])); c->stage_ms[FSLIC_T_CIELAB] = ms;
         CK(cudaEventElapsedTime(&ms, c->ev[1], c->ev[2])); c->stage_ms[FSLIC_T_ASSIGN] = ms;
         c->stage_ms[FSLIC_T_UPDATE] = 0.f;  // fused into assign
+        c->stage_ms[FSLIC_T_BEFORE_ITERATION] = 0.f;
+        c->stage_ms[FSLIC_T_AFTER_UPDATE] = 0.f;
+        if (variant == 4) {  // LSC: before_iteration and the after_update launches are their own stages
+            CK(cudaEventElapsedTime(&ms, c->ev[1], c->ev[5])); c->stage_ms[FSLIC_T_BEFORE_ITERATION] = ms;
+            CK(cudaEventElapsedTime(&ms, c->ev[5], c->ev[2])); c->stage_ms[FSLIC_T_ASSIGN] = ms;
+            for (int i = 0; i + 1 < c->lev_used; i += 2) {
+                CK(cudaEventElapsedTime(&ms, c->lev[i], c->lev[i + 1]));
+                c->stage_ms[FSLIC_T_AFTER_UPDATE] += ms;
+            }
+            c->stage_ms[FSLIC_T_ASSIGN] -= c->stage_ms[FSLIC_T_AFTER_UPDATE];
+        }
         CK(cudaEventElapsedTime(&ms, c->ev[2], c->ev[3])); c->stage_ms[FSLIC_T_FULL_ASSIGN] = ms;
         CK(cudaEventElapsedTime(&ms, c->ev[3], c->ev[4])); c->stage_ms[FSLIC_T_CCA] = ms;
         CK(cudaEventElapsedTime(&ms, c->ev[0], c->ev[4])); c->stage_ms[FSLIC_T_TOTAL] = ms;
@@ -1132,6 +1295,34 @@ extern "C" int fslic_b200_iterate_real(fslic_ctx* c, int variant, const uint8_t*
                                        uint16_t* d_labels, int batch, const fslic_params* p, void* stream) {
     if (variant < 0 || variant > 2) return set_err(FSLIC_EINVAL, "variant must be 0 (standard), 1 (l2) or 2 (noq)");
     return iterate_plain(c, d_images, d_clusters, d_labels, batch, p, stream, false, variant);
+}
+
+// The reference's ContextLSC (src/lsc.cpp; cfast_slic.pyx:207-214) driven with num_threads = 1 (lsc.cuh).
+extern "C" int fslic_b200_iterate_lsc(fslic_ctx* c, const uint8_t* d_images, fslic_cluster* d_clusters, uint16_t* d_labels,
+                                      int batch, const fslic_params* p, void* stream) {
+    int rc = check_batch(c, batch);
+    if (rc) return rc;
+    USE_DEVICE(c->device);
+    rc = ensure_lsc(c);
+    if (rc) return rc;
+    return iterate_plain(c, d_images, d_clusters, d_labels, batch, p, stream, false, 4);
+}
+
+extern "C" int fslic_b200_debug_lsc_stages(fslic_ctx* c, float* d_means_out, float* d_weights_out, float* d_cinit_out,
+                                           int batch, void* stream) {
+    int rc = check_batch(c, batch);
+    if (rc) return rc;
+    if (!c->lsc_feat) return set_err(FSLIC_EINVAL, "no LSC iterate has run on this context");
+    USE_DEVICE(c->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (d_means_out)
+        CK(cudaMemcpyAsync(d_means_out, c->lsc_means, sizeof(float) * LSC_NF * batch, cudaMemcpyDeviceToDevice, st));
+    if (d_weights_out)
+        CK(cudaMemcpyAsync(d_weights_out, c->lsc_w, sizeof(float) * (size_t)c->N * batch, cudaMemcpyDeviceToDevice, st));
+    if (d_cinit_out)
+        CK(cudaMemcpyAsync(d_cinit_out, c->lsc_cf_init, sizeof(float) * LSC_NF * (size_t)c->K * batch,
+                           cudaMemcpyDeviceToDevice, st));
+    return FSLIC_OK;
 }
 
 extern "C" int fslic_b200_iterate_preemptive(fslic_ctx* c, const uint8_t* d_images, fslic_cluster* d_clusters, uint16_t* d_labels,

@@ -135,6 +135,29 @@ class Engine:
                                                         C.byref(params), C.c_float(preemptive_thres), _stream_ptr(self.device)))
         return labels
 
+    def iterate_lsc(self, images, clusters, params, labels=None, manhattan_spatial_dist=True):
+        """LSC, linear spectral clustering (fslic_b200_iterate_lsc): the reference's ContextLSC with num_threads = 1;
+        device tensors like iterate().  manhattan_spatial_dist is accepted and has no effect, as in the reference."""
+        self._check_images(images)
+        B = images.shape[0]
+        if labels is None:
+            labels = torch.empty((B, self.H, self.W), dtype=torch.int16, device=self.device)
+        with self.lock:
+            self._set_spatial(manhattan_spatial_dist)
+            check(self._L.fslic_b200_iterate_lsc(self._h, images.data_ptr(), clusters.data_ptr(), labels.data_ptr(), B,
+                                                 C.byref(params), _stream_ptr(self.device)))
+        return labels
+
+    def debug_lsc_stages(self, batch):
+        """(means float32[B,10], weights float32[B,H,W], initial centroid features float32[B,K,10]) of the last
+        iterate_lsc."""
+        means = torch.empty((batch, 10), dtype=torch.float32, device=self.device)
+        weights = torch.empty((batch, self.H, self.W), dtype=torch.float32, device=self.device)
+        cinit = torch.empty((batch, self.K, 10), dtype=torch.float32, device=self.device)
+        check(self._L.fslic_b200_debug_lsc_stages(self._h, means.data_ptr(), weights.data_ptr(), cinit.data_ptr(), batch,
+                                                  _stream_ptr(self.device)))
+        return means, weights, cinit
+
     def enforce_connectivity(self, labels, K, min_threshold):
         """In place on int16/uint16 labels [B,H,W] (cuda)."""
         B = labels.shape[0]
@@ -199,6 +222,12 @@ class Engine:
         out = (C.c_float * 6)()
         check(self._L.fslic_b200_stage_ms(self._h, out, 6))
         return dict(zip(_lib.STAGE_NAMES, [float(v) for v in out]))
+
+    def lsc_stage_ms(self):
+        """before_iteration / after_update milliseconds of the last timed iterate_lsc (zero after other calls)."""
+        out = (C.c_float * 8)()
+        check(self._L.fslic_b200_stage_ms(self._h, out, 8))
+        return dict(zip(_lib.LSC_STAGE_NAMES, [float(v) for v in out[6:8]]))
 
     def cca_stage_ms(self):
         out = (C.c_float * 6)()

@@ -60,7 +60,9 @@ typedef struct fslic_ctx fslic_ctx;
  * (context.cpp:112-192, cca.cpp:194-259). */
 enum {
     FSLIC_T_CIELAB = 0, FSLIC_T_ASSIGN = 1, FSLIC_T_UPDATE = 2, FSLIC_T_FULL_ASSIGN = 3,
-    FSLIC_T_CCA = 4, FSLIC_T_TOTAL = 5, FSLIC_T_COUNT = 6
+    FSLIC_T_CCA = 4, FSLIC_T_TOTAL = 5,
+    FSLIC_T_BEFORE_ITERATION = 6, FSLIC_T_AFTER_UPDATE = 7, /* LSC only (zero otherwise), lsc.cpp:12-15,226-307 */
+    FSLIC_T_COUNT = 8
 };
 
 const char* fslic_b200_last_error(void);
@@ -110,6 +112,22 @@ int fslic_b200_iterate_real(fslic_ctx* ctx, int variant, const uint8_t* d_images
  *    countdown where it got to.  Same buffers as fslic_b200_iterate; bit-identical to the reference.  S >= 1. */
 int fslic_b200_iterate_preemptive(fslic_ctx* ctx, const uint8_t* d_images, fslic_cluster* d_clusters, uint16_t* d_labels,
                                   int batch, const fslic_params* params, float preemptive_thres, void* stream);
+
+/* == the reference's ContextLSC (src/lsc.cpp, lsc.h: linear spectral clustering; cfast_slic.pyx:207-214, arch
+ *    "standard") run with num_threads = 1 -- the only thread count at which the reference's result is defined: its
+ *    after_update merges per-thread partial sums in arrival order.  Ten per-pixel features (L, a, b and x, y mapped
+ *    onto quarter circles), weighted by their means; assign by the squared 10-D distance over the (2S+1)^2 window;
+ *    integer Cluster update as fslic_b200_iterate, plus weighted 10-D centroid features.  Same buffers and
+ *    semantics as fslic_b200_iterate; labels, pre-CCA labels and Cluster records bit-identical to the reference.
+ *    manhattan_spatial_dist has no effect.  The first call allocates about 44 bytes per pixel of max_batch images. */
+int fslic_b200_iterate_lsc(fslic_ctx* ctx, const uint8_t* d_images, fslic_cluster* d_clusters, uint16_t* d_labels,
+                           int batch, const fslic_params* params, void* stream);
+
+/* Stage probes of the last fslic_b200_iterate_lsc (before_iteration, lsc.cpp:22-195), into caller device buffers (any
+ * may be NULL): the feature means float[B][10], the pixel weights float[B][H][W] and the initial centroid features
+ * float[B][K][10]. */
+int fslic_b200_debug_lsc_stages(fslic_ctx* ctx, float* d_means_out, float* d_weights_out, float* d_cinit_out, int batch,
+                                void* stream);
 
 /* The same call as the reference-facing plugin makes it: HOST buffers in, HOST buffers out
  * (what SlicModel.iterate does with a numpy image, cfast_slic.pyx:150-260).  H2D copy, kernels and
