@@ -21,6 +21,13 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_get_mask_density", "fslic_b200_cluster_density_to_mask", "fslic_b200_cca_stage_ms",
     "fslic_b200_iterate_real", "fslic_b200_iterate_preemptive", "fslic_b200_set_manhattan_spatial_dist",
     "fslic_b200_iterate_lsc", "fslic_b200_debug_lsc_stages",
+    "fslic_b200_crf_create", "fslic_b200_crf_destroy", "fslic_b200_crf_get_params", "fslic_b200_crf_set_params",
+    "fslic_b200_crf_times", "fslic_b200_crf_push_frame", "fslic_b200_crf_pop_frame", "fslic_b200_crf_set_clusters",
+    "fslic_b200_crf_get_clusters", "fslic_b200_crf_set_connectivity", "fslic_b200_crf_get_connectivity",
+    "fslic_b200_crf_set_unary", "fslic_b200_crf_get_unary", "fslic_b200_crf_set_unbiased", "fslic_b200_crf_set_mask",
+    "fslic_b200_crf_set_proba", "fslic_b200_crf_get_inferred", "fslic_b200_crf_reset_inferred",
+    "fslic_b200_crf_initialize", "fslic_b200_crf_inference", "fslic_b200_crf_spatial_pairwise_energy",
+    "fslic_b200_crf_temporal_pairwise_energy", "fslic_b200_debug_expf_host", "fslic_b200_debug_expf_device",
 )
 
 STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity", "iterate")

@@ -7,6 +7,7 @@
 #include <stdlib.h>
 #include <new>
 #include <cstring>
+#include <deque>
 #include <string>
 #include <vector>
 
@@ -17,6 +18,7 @@
 #include "graph.cuh"
 #include "realdist.cuh"
 #include "lsc.cuh"
+#include "crf.cuh"
 #include "preempt.cuh"
 #include "cca.cuh"
 #include "common.cuh"
@@ -1807,6 +1809,476 @@ extern "C" int fslic_b200_cluster_density_to_mask(int device, int H, int W, int 
     const long cap = grid_stride_cap(device);
     if (blocks > cap) blocks = cap;
     k_density_broadcast<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(d_labels, d_densities, n, K, d_result);
+    CK(cudaGetLastError());
+    return FSLIC_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// SimpleCRF (src/simple-crf.{h,hpp,cpp}; csimple_crf.pyx).  The frames live in a deque in time order, exactly like the
+// reference's; each owns its device buffers (crf.cuh) plus host copies of its clusters and adjacency lists, which the
+// getters and the pairwise-energy queries read.  Slots of popped frames are kept and reused by the next push.
+// Every copy, memset and kernel of a CRF goes to the CRF's stream (the last one passed to inference, NULL at first), so
+// they are ordered whatever kind of stream that is.  inference / initialize / reset_inferred return at once; every
+// other entry point synchronises that stream before it returns.
+struct CrfSlot {
+    int time = 0;
+    fslic_cluster* clusters = nullptr;
+    int32_t* offsets = nullptr;
+    int32_t* nbr = nullptr;
+    float* e_sp = nullptr;
+    float* r_sp = nullptr;
+    size_t edge_cap = 0;
+    float *unary = nullptr, *q0 = nullptr, *q1 = nullptr, *msg = nullptr, *tmp = nullptr;
+    std::vector<fslic_cluster> h_clusters;
+    std::vector<int32_t> h_off, h_nbr;
+};
+
+struct fslic_crf {
+    int device = 0, C = 0, N = 0;
+    CrfParams p{};
+    int next_time = 0, cur = 0;
+    std::deque<CrfSlot*> frames;
+    std::vector<CrfSlot*> pool;
+    CrfFrameDev* d_table = nullptr;
+    size_t table_cap = 0;
+    float* d_scalar = nullptr;
+    cudaStream_t st = nullptr;
+};
+
+static void crf_free_slot(CrfSlot* s) {
+    cudaFree(s->clusters); cudaFree(s->offsets); cudaFree(s->nbr); cudaFree(s->e_sp); cudaFree(s->r_sp);
+    cudaFree(s->unary); cudaFree(s->q0); cudaFree(s->q1); cudaFree(s->msg); cudaFree(s->tmp);
+    delete s;
+}
+
+#define CKA(call)                                                                                     \
+    do {                                                                                              \
+        cudaError_t e__ = (call);                                                                     \
+        if (e__ != cudaSuccess)                                                                       \
+            return set_err(e__ == cudaErrorMemoryAllocation ? FSLIC_ENOMEM : FSLIC_ECUDA,              \
+                           std::string(#call) + ": " + cudaGetErrorString(e__));                      \
+    } while (0)
+
+static int crf_upload_table(fslic_crf* c) {
+    const size_t T = c->frames.size();
+    if (T > c->table_cap) {
+        cudaFree(c->d_table);
+        c->d_table = nullptr;
+        c->table_cap = 0;
+        CKA(cudaMalloc(&c->d_table, sizeof(CrfFrameDev) * T * 2));
+        c->table_cap = T * 2;
+    }
+    std::vector<CrfFrameDev> h(T);
+    for (size_t t = 0; t < T; t++) {
+        const CrfSlot* s = c->frames[t];
+        h[t] = CrfFrameDev{s->clusters, s->offsets, s->nbr, s->unary, {s->q0, s->q1}, s->msg, s->e_sp, s->r_sp, s->tmp};
+    }
+    if (T) CK(cudaMemcpyAsync(c->d_table, h.data(), sizeof(CrfFrameDev) * T, cudaMemcpyHostToDevice, c->st));
+    CK(cudaStreamSynchronize(c->st));
+    return FSLIC_OK;
+}
+
+static int crf_frame(fslic_crf* c, int time, CrfSlot** out) {
+    if (!c) return set_err(FSLIC_EINVAL, "crf is NULL");
+    if (c->frames.empty() || time < c->frames.front()->time || time > c->frames.back()->time)
+        return set_err(FSLIC_ENOFRAME, "Time out of range");  // SimpleCRF::get_frame (simple-crf.hpp:111-119)
+    *out = c->frames[(size_t)(time - c->frames.front()->time)];
+    return FSLIC_OK;
+}
+
+// Look up the frame `time`, switch to the CRF's device and wait for its stream.
+#define CRF_FRAME(c, time, s)                                                                         \
+    CrfSlot* s = nullptr;                                                                             \
+    { int rc__ = crf_frame(c, time, &s); if (rc__) return rc__; }                                     \
+    USE_DEVICE((c)->device);                                                                          \
+    CK(cudaStreamSynchronize((c)->st))
+
+extern "C" int fslic_b200_crf_create(int device, int num_classes, int num_nodes, fslic_crf** out) {
+    if (!out) return set_err(FSLIC_EINVAL, "out is NULL");
+    *out = nullptr;
+    if (num_classes < 0 || num_nodes < 0) return set_err(FSLIC_EINVAL, "num_classes and num_nodes must be >= 0");
+    if ((long long)num_classes * num_nodes > (1LL << 31) - 1)
+        return set_err(FSLIC_EINVAL, "num_classes * num_nodes must be < 2^31");
+    USE_DEVICE(device);
+    fslic_crf* c = new (std::nothrow) fslic_crf();
+    if (!c) return set_err(FSLIC_ENOMEM, "out of host memory");
+    c->device = device;
+    c->C = num_classes;
+    c->N = num_nodes;
+    c->p = CrfParams{10, 10, 13, 13, 80, 0, 3};  // SimpleCRF::SimpleCRF (simple-crf.hpp:80-89)
+    cudaError_t e = cudaMalloc(&c->d_scalar, sizeof(float));
+    if (e != cudaSuccess) {
+        delete c;
+        return set_err(e == cudaErrorMemoryAllocation ? FSLIC_ENOMEM : FSLIC_ECUDA,
+                       std::string("cudaMalloc: ") + cudaGetErrorString(e));
+    }
+    *out = c;
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_crf_destroy(fslic_crf* c) {
+    if (!c) return FSLIC_OK;
+    DeviceGuard dev_guard__(c->device);
+    cudaStreamSynchronize(c->st);
+    for (CrfSlot* s : c->frames) crf_free_slot(s);
+    for (CrfSlot* s : c->pool) crf_free_slot(s);
+    cudaFree(c->d_table);
+    cudaFree(c->d_scalar);
+    delete c;
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_crf_get_params(const fslic_crf* c, fslic_crf_params* out) {
+    if (!c || !out) return set_err(FSLIC_EINVAL, "NULL argument");
+    static_assert(sizeof(CrfParams) == sizeof(fslic_crf_params), "params layout");
+    memcpy(out, &c->p, sizeof(CrfParams));
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_crf_set_params(fslic_crf* c, const fslic_crf_params* params) {
+    if (!c || !params) return set_err(FSLIC_EINVAL, "NULL argument");
+    memcpy(&c->p, params, sizeof(CrfParams));  // read by the next inference() when it enqueues
+    return FSLIC_OK;
+}
+
+// first_time, last_time (-1 when there are no frames) and the number of frames
+extern "C" int fslic_b200_crf_times(const fslic_crf* c, int* first, int* last, int* num_frames) {
+    if (!c) return set_err(FSLIC_EINVAL, "crf is NULL");
+    if (first) *first = c->frames.empty() ? -1 : c->frames.front()->time;
+    if (last) *last = c->frames.empty() ? -1 : c->frames.back()->time;
+    if (num_frames) *num_frames = (int)c->frames.size();
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_crf_push_frame(fslic_crf* c, int* time_out) {
+    if (!c) return set_err(FSLIC_EINVAL, "crf is NULL");
+    USE_DEVICE(c->device);
+    CK(cudaStreamSynchronize(c->st));
+    const size_t N = (size_t)c->N, CN = (size_t)c->C * c->N;
+    CrfSlot* s;
+    if (!c->pool.empty()) {
+        s = c->pool.back();
+        c->pool.pop_back();
+    } else {
+        s = new (std::nothrow) CrfSlot();
+        if (!s) return set_err(FSLIC_ENOMEM, "out of host memory");
+        cudaError_t e = cudaSuccess;
+        if (e == cudaSuccess && N) e = cudaMalloc(&s->clusters, sizeof(fslic_cluster) * N);
+        if (e == cudaSuccess) e = cudaMalloc(&s->offsets, sizeof(int32_t) * (N + 1));
+        if (e == cudaSuccess && CN) e = cudaMalloc(&s->unary, sizeof(float) * CN);
+        if (e == cudaSuccess && CN) e = cudaMalloc(&s->q0, sizeof(float) * CN);
+        if (e == cudaSuccess && CN) e = cudaMalloc(&s->q1, sizeof(float) * CN);
+        if (e == cudaSuccess && CN) e = cudaMalloc(&s->msg, sizeof(float) * CN);
+        if (e == cudaSuccess && N) e = cudaMalloc(&s->tmp, sizeof(float) * 4 * N);
+        if (e != cudaSuccess) {
+            crf_free_slot(s);
+            return set_err(e == cudaErrorMemoryAllocation ? FSLIC_ENOMEM : FSLIC_ECUDA,
+                           std::string("cudaMalloc: ") + cudaGetErrorString(e));
+        }
+    }
+    // SimpleCRFFrame::SimpleCRFFrame (simple-crf.hpp:29-33): value-initialised clusters with num_members = 1, empty
+    // adjacency lists, unaries and q zero
+    fslic_cluster blank;
+    memset(&blank, 0, sizeof(blank));
+    blank.num_members = 1;
+    s->h_clusters.assign(N, blank);
+    s->h_off.assign(N + 1, 0);
+    s->h_nbr.clear();
+    if (N) CK(cudaMemcpyAsync(s->clusters, s->h_clusters.data(), sizeof(fslic_cluster) * N, cudaMemcpyHostToDevice, c->st));
+    CK(cudaMemsetAsync(s->offsets, 0, sizeof(int32_t) * (N + 1), c->st));
+    if (CN) {
+        CK(cudaMemsetAsync(s->unary, 0, sizeof(float) * CN, c->st));
+        CK(cudaMemsetAsync(s->q0, 0, sizeof(float) * CN, c->st));
+        CK(cudaMemsetAsync(s->q1, 0, sizeof(float) * CN, c->st));
+    }
+    s->time = c->next_time++;
+    c->frames.push_back(s);
+    int rc = crf_upload_table(c);
+    if (rc) {
+        c->frames.pop_back();
+        c->pool.push_back(s);
+        c->next_time--;
+        return rc;
+    }
+    if (time_out) *time_out = s->time;
+    return FSLIC_OK;
+}
+
+// SimpleCRF::pop_frame (simple-crf.hpp:103-109): drops the first frame; *time_out = its time, -1 when empty
+extern "C" int fslic_b200_crf_pop_frame(fslic_crf* c, int* time_out) {
+    if (!c) return set_err(FSLIC_EINVAL, "crf is NULL");
+    if (c->frames.empty()) {
+        if (time_out) *time_out = -1;
+        return FSLIC_OK;
+    }
+    USE_DEVICE(c->device);
+    CK(cudaStreamSynchronize(c->st));
+    CrfSlot* s = c->frames.front();
+    c->frames.pop_front();
+    c->pool.push_back(s);
+    if (time_out) *time_out = s->time;
+    return crf_upload_table(c);
+}
+
+extern "C" int fslic_b200_crf_set_clusters(fslic_crf* c, int time, const fslic_cluster* h_clusters) {
+    if (!h_clusters && c && c->N) return set_err(FSLIC_EINVAL, "NULL argument");
+    CRF_FRAME(c, time, s);
+    if (c->N) {
+        memcpy(s->h_clusters.data(), h_clusters, sizeof(fslic_cluster) * c->N);
+        CK(cudaMemcpyAsync(s->clusters, h_clusters, sizeof(fslic_cluster) * c->N, cudaMemcpyHostToDevice, c->st));
+        CK(cudaStreamSynchronize(c->st));
+    }
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_crf_get_clusters(fslic_crf* c, int time, fslic_cluster* h_out) {
+    CrfSlot* s = nullptr;
+    int rc = crf_frame(c, time, &s);
+    if (rc) return rc;
+    if (c->N) memcpy(h_out, s->h_clusters.data(), sizeof(fslic_cluster) * c->N);
+    return FSLIC_OK;
+}
+
+// SimpleCRFFrame::set_connectivity (simple-crf.cpp:11-19): rows 0..num_rows-1 get the lists of the CSR (h_offsets
+// [num_rows + 1], h_neighbors [h_offsets[num_rows]]), the other rows keep theirs.  Every neighbour must be a node of
+// the frame; otherwise nothing changes.
+extern "C" int fslic_b200_crf_set_connectivity(fslic_crf* c, int time, int num_rows, const int32_t* h_offsets,
+                                               const int32_t* h_neighbors) {
+    CrfSlot* s = nullptr;
+    int rc = crf_frame(c, time, &s);
+    if (rc) return rc;
+    const int N = c->N;
+    if (num_rows < 0 || num_rows > N) return set_err(FSLIC_EINVAL, "more adjacency lists than nodes");
+    if (!h_offsets) return set_err(FSLIC_EINVAL, "NULL argument");
+    if (h_offsets[0] != 0) return set_err(FSLIC_EINVAL, "offsets must start at 0");
+    for (int i = 0; i < num_rows; i++)
+        if (h_offsets[i + 1] < h_offsets[i]) return set_err(FSLIC_EINVAL, "offsets must not decrease");
+    const int32_t E_new = h_offsets[num_rows];
+    if (E_new && !h_neighbors) return set_err(FSLIC_EINVAL, "NULL argument");
+    for (int32_t k = 0; k < E_new; k++)
+        if (h_neighbors[k] < 0 || h_neighbors[k] >= N)
+            return set_err(FSLIC_EINVAL, "neighbour index out of range");
+    std::vector<int32_t> off(N + 1), nb;
+    const long long E = (long long)E_new + (s->h_off[N] - s->h_off[num_rows]);
+    if (E > (1LL << 31) - 1) return set_err(FSLIC_EINVAL, "too many edges");
+    nb.reserve((size_t)E);
+    nb.insert(nb.end(), h_neighbors, h_neighbors + E_new);
+    memcpy(off.data(), h_offsets, sizeof(int32_t) * (num_rows + 1));
+    nb.insert(nb.end(), s->h_nbr.begin() + s->h_off[num_rows], s->h_nbr.end());
+    for (int i = num_rows; i < N; i++) off[i + 1] = off[i] + (s->h_off[i + 1] - s->h_off[i]);
+    USE_DEVICE(c->device);
+    CK(cudaStreamSynchronize(c->st));
+    if ((size_t)E > s->edge_cap) {
+        cudaFree(s->nbr); cudaFree(s->e_sp); cudaFree(s->r_sp);
+        s->nbr = nullptr; s->e_sp = s->r_sp = nullptr; s->edge_cap = 0;
+        s->h_off.assign(N + 1, 0);  // until the new lists are in place the frame has none
+        s->h_nbr.clear();
+        CKA(cudaMemsetAsync(s->offsets, 0, sizeof(int32_t) * (N + 1), c->st));
+        const size_t cap = (size_t)E + (size_t)E / 2;
+        CKA(cudaMalloc(&s->nbr, sizeof(int32_t) * cap));
+        CKA(cudaMalloc(&s->e_sp, sizeof(float) * cap));
+        CKA(cudaMalloc(&s->r_sp, sizeof(float) * cap));
+        s->edge_cap = cap;
+        rc = crf_upload_table(c);
+        if (rc) return rc;
+    }
+    if (E) CK(cudaMemcpyAsync(s->nbr, nb.data(), sizeof(int32_t) * E, cudaMemcpyHostToDevice, c->st));
+    CK(cudaMemcpyAsync(s->offsets, off.data(), sizeof(int32_t) * (N + 1), cudaMemcpyHostToDevice, c->st));
+    CK(cudaStreamSynchronize(c->st));
+    s->h_off.swap(off);
+    s->h_nbr.swap(nb);
+    return FSLIC_OK;
+}
+
+// The adjacency lists as CSR: h_offsets [N + 1]; h_neighbors (may be NULL) receives the first `cap` neighbours.
+extern "C" int fslic_b200_crf_get_connectivity(fslic_crf* c, int time, int32_t* h_offsets, int32_t* h_neighbors,
+                                               long long cap) {
+    CrfSlot* s = nullptr;
+    int rc = crf_frame(c, time, &s);
+    if (rc) return rc;
+    if (h_offsets) memcpy(h_offsets, s->h_off.data(), sizeof(int32_t) * (c->N + 1));
+    if (h_neighbors) {
+        const size_t n = std::min((size_t)(cap < 0 ? 0 : cap), s->h_nbr.size());
+        if (n) memcpy(h_neighbors, s->h_nbr.data(), sizeof(int32_t) * n);
+    }
+    return FSLIC_OK;
+}
+
+static int crf_put_unary(fslic_crf* c, CrfSlot* s, const float* h) {
+    const size_t CN = (size_t)c->C * c->N;
+    if (CN) CK(cudaMemcpyAsync(s->unary, h, sizeof(float) * CN, cudaMemcpyHostToDevice, c->st));
+    CK(cudaStreamSynchronize(c->st));
+    return FSLIC_OK;
+}
+
+// SimpleCRFFrame::set_unary / get_unary (simple-crf.hpp:53-61): float [C][N]
+extern "C" int fslic_b200_crf_set_unary(fslic_crf* c, int time, const float* h_unary) {
+    CRF_FRAME(c, time, s);
+    return crf_put_unary(c, s, h_unary);
+}
+
+extern "C" int fslic_b200_crf_get_unary(fslic_crf* c, int time, float* h_out) {
+    CRF_FRAME(c, time, s);
+    const size_t CN = (size_t)c->C * c->N;
+    if (CN) CK(cudaMemcpyAsync(h_out, s->unary, sizeof(float) * CN, cudaMemcpyDeviceToHost, c->st));
+    CK(cudaStreamSynchronize(c->st));
+    return FSLIC_OK;
+}
+
+// The unary setters run on the host with glibc's logf, as the reference's do.  Their float arithmetic is the object
+// code's: set_mask's active probability is one fused multiply-add.
+// SimpleCRFFrame::set_unbiased (simple-crf.cpp:34-37)
+extern "C" int fslic_b200_crf_set_unbiased(fslic_crf* c, int time) {
+    CRF_FRAME(c, time, s);
+    std::vector<float> u((size_t)c->C * c->N, logf((float)c->C));
+    return crf_put_unary(c, s, u.data());
+}
+
+// SimpleCRFFrame::set_mask (simple-crf.cpp:39-50).  Every class must be in [0, C); otherwise nothing changes.
+extern "C" int fslic_b200_crf_set_mask(fslic_crf* c, int time, const int32_t* h_classes, float confidence) {
+    CRF_FRAME(c, time, s);
+    const int C = c->C, N = c->N;
+    for (int i = 0; i < N; i++)
+        if (h_classes[i] < 0 || h_classes[i] >= C) return set_err(FSLIC_EINVAL, "class index out of range");
+    const float lowest = 1.0f / (float)C;
+    const float active = fmaf(1.0f - lowest, confidence, lowest);
+    const float inactive = (1.0f - active) / (float)(C - 1);
+    const float active_unary = -logf(active), inactive_unary = -logf(inactive);
+    std::vector<float> u((size_t)C * N, inactive_unary);
+    for (int i = 0; i < N; i++) u[(size_t)N * h_classes[i] + i] = active_unary;
+    return crf_put_unary(c, s, u.data());
+}
+
+// SimpleCRFFrame::set_proba (simple-crf.cpp:53-55): unary = -logf(p), p float [C][N]
+extern "C" int fslic_b200_crf_set_proba(fslic_crf* c, int time, const float* h_proba) {
+    CRF_FRAME(c, time, s);
+    const size_t CN = (size_t)c->C * c->N;
+    std::vector<float> u(CN);
+    for (size_t k = 0; k < CN; k++) u[k] = -logf(h_proba[k]);
+    return crf_put_unary(c, s, u.data());
+}
+
+// SimpleCRFFrame::get_inferred: q float [C][N]
+extern "C" int fslic_b200_crf_get_inferred(fslic_crf* c, int time, float* h_out) {
+    CRF_FRAME(c, time, s);
+    const size_t CN = (size_t)c->C * c->N;
+    if (CN) CK(cudaMemcpyAsync(h_out, c->cur ? s->q1 : s->q0, sizeof(float) * CN, cudaMemcpyDeviceToHost, c->st));
+    CK(cudaStreamSynchronize(c->st));
+    return FSLIC_OK;
+}
+
+static int crf_reset(fslic_crf* c, CrfSlot* s) {
+    const long long CN = (long long)c->C * c->N;
+    if (!CN) return FSLIC_OK;
+    k_crf_reset<<<(unsigned)((CN + 255) / 256), 256, 0, c->st>>>(s->unary, c->cur ? s->q1 : s->q0, CN);
+    CK(cudaGetLastError());
+    return FSLIC_OK;
+}
+
+// SimpleCRFFrame::reset_inferred (simple-crf.cpp:57-59): q = expf(-unary), asynchronous on the CRF's stream
+extern "C" int fslic_b200_crf_reset_inferred(fslic_crf* c, int time) {
+    CrfSlot* s = nullptr;
+    int rc = crf_frame(c, time, &s);
+    if (rc) return rc;
+    USE_DEVICE(c->device);
+    return crf_reset(c, s);
+}
+
+// SimpleCRF::initialize (simple-crf.cpp:153-157): reset_inferred on every frame
+extern "C" int fslic_b200_crf_initialize(fslic_crf* c) {
+    if (!c) return set_err(FSLIC_EINVAL, "crf is NULL");
+    USE_DEVICE(c->device);
+    for (CrfSlot* s : c->frames) {
+        int rc = crf_reset(c, s);
+        if (rc) return rc;
+    }
+    return FSLIC_OK;
+}
+
+// SimpleCRF::inference (simple-crf.cpp:159-163): max_iter Jacobi steps over all frames.  1 + 2 max_iter launches on
+// `stream`, no host synchronisation.  With no frames the reference's infer_once looks up time -1 and throws
+// std::out_of_range; here that is FSLIC_ENOFRAME.
+extern "C" int fslic_b200_crf_inference(fslic_crf* c, unsigned long long max_iter, void* stream) {
+    if (!c) return set_err(FSLIC_EINVAL, "crf is NULL");
+    if (max_iter == 0) return FSLIC_OK;
+    if (c->frames.empty()) return set_err(FSLIC_ENOFRAME, "Time out of range");
+    USE_DEVICE(c->device);
+    if ((cudaStream_t)stream != c->st) {
+        CK(cudaStreamSynchronize(c->st));
+        c->st = (cudaStream_t)stream;
+    }
+    const long long TN = (long long)c->frames.size() * c->N;
+    if (!TN || !c->C) return FSLIC_OK;
+    const int T = (int)c->frames.size();
+    const unsigned blocks = (unsigned)((TN + 127) / 128);
+    k_crf_pairwise<<<blocks, 128, 0, c->st>>>(c->d_table, T, c->N, c->p);
+    CK(cudaGetLastError());
+    const long long TCN = TN * c->C;
+    for (unsigned long long it = 0; it < max_iter; it++) {
+        k_crf_msg<<<(unsigned)((TCN + 127) / 128), 128, 0, c->st>>>(c->d_table, T, c->N, c->C, c->cur);
+        k_crf_compat<<<blocks, 128, 0, c->st>>>(c->d_table, T, c->N, c->C, c->cur);
+        CK(cudaGetLastError());
+        c->cur ^= 1;
+    }
+    return FSLIC_OK;
+}
+
+// SimpleCRFFrame::calc_spatial_pairwise_energy(node_i, node_j) of frame `time` (simple-crf.hpp:149-174)
+extern "C" int fslic_b200_crf_spatial_pairwise_energy(fslic_crf* c, int time, int node_i, int node_j, float* out) {
+    CRF_FRAME(c, time, s);
+    if (node_i < 0 || node_j < 0 || node_i >= c->N || node_j >= c->N) return set_err(FSLIC_EINVAL, "node number is out of range");
+    if (node_i == node_j) {
+        *out = 0.0f;
+        return FSLIC_OK;
+    }
+    k_crf_energy<<<1, 1, 0, c->st>>>(s->h_clusters[node_i], s->h_clusters[node_j], 1, c->p, c->d_scalar);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(out, c->d_scalar, sizeof(float), cudaMemcpyDeviceToHost, c->st));
+    CK(cudaStreamSynchronize(c->st));
+    return FSLIC_OK;
+}
+
+// SimpleCRFFrame::calc_temporal_pairwise_energy(node, other) of frame `time` of `c` against frame `other_time` of `other`
+// (simple-crf.hpp:135-147), with c's params; 0 when both are the same frame.
+extern "C" int fslic_b200_crf_temporal_pairwise_energy(fslic_crf* c, int time, int node, fslic_crf* other, int other_time,
+                                                       float* out) {
+    CrfSlot* o = nullptr;
+    int rc = crf_frame(other, other_time, &o);
+    if (rc) return rc;
+    CRF_FRAME(c, time, s);
+    if (node < 0 || node >= c->N || node >= other->N) return set_err(FSLIC_EINVAL, "node number is out of range");
+    if (s == o) {
+        *out = 0.0f;
+        return FSLIC_OK;
+    }
+    k_crf_energy<<<1, 1, 0, c->st>>>(s->h_clusters[node], o->h_clusters[node], 0, c->p, c->d_scalar);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(out, c->d_scalar, sizeof(float), cudaMemcpyDeviceToHost, c->st));
+    CK(cudaStreamSynchronize(c->st));
+    return FSLIC_OK;
+}
+
+// The expf clone of glibc_expf.cuh over the bit patterns first .. first + n - 1 (wrapping), host and device compiles.
+__attribute__((target("fma"))) static void expf_host_fma(uint32_t first, long long n, float* out) {
+    for (long long i = 0; i < n; i++) out[i] = gexpf::expf(gexpf::u2f(first + (uint32_t)i));
+}
+static void expf_host_generic(uint32_t first, long long n, float* out) {
+    for (long long i = 0; i < n; i++) out[i] = gexpf::expf(gexpf::u2f(first + (uint32_t)i));
+}
+
+extern "C" int fslic_b200_debug_expf_host(uint32_t first, long long n, float* h_out) {
+    if (n < 0 || (n && !h_out)) return set_err(FSLIC_EINVAL, "bad buffer");
+    // both are exact (libm's fma is correctly rounded); the FMA instruction is only faster
+    if (__builtin_cpu_supports("fma")) expf_host_fma(first, n, h_out);
+    else expf_host_generic(first, n, h_out);
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_debug_expf_device(int device, uint32_t first, long long n, float* d_out, void* stream) {
+    if (n < 0 || (n && !d_out)) return set_err(FSLIC_EINVAL, "bad buffer");
+    if (!n) return FSLIC_OK;
+    USE_DEVICE(device);
+    k_expf_debug<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(first, n, d_out);
     CK(cudaGetLastError());
     return FSLIC_OK;
 }

@@ -51,7 +51,8 @@ enum {
     FSLIC_EINVAL = -1,   /* bad argument (reference: ValueError, cfast_slic.pyx:24-27,125,153) */
     FSLIC_ECUDA = -2,    /* CUDA runtime error */
     FSLIC_ENOMEM = -3,
-    FSLIC_ERANGE = -4    /* compactness so large the u16 distance would overflow (UB in the reference) */
+    FSLIC_ERANGE = -4,   /* compactness so large the u16 distance would overflow (UB in the reference) */
+    FSLIC_ENOFRAME = -5  /* CRF: no frame with that time (reference: std::out_of_range, IndexError in Python) */
 };
 
 typedef struct fslic_ctx fslic_ctx;
@@ -211,6 +212,60 @@ int fslic_b200_launches_last_iterate(const fslic_ctx* ctx);
  * (k_assign5; needs W % 8 == 0 and subsample_stride 3), 4: the LDG kernel (k_assign_warp; any shape; forced
  * by the environment variable FSLIC_ASSIGN=4 at context creation), 0: the brute-force kernel / none yet. */
 int fslic_b200_debug_assign_impl(const fslic_ctx* ctx);
+
+/* ---- SimpleCRF (src/simple-crf.{h,hpp,cpp}, csimple_crf.pyx): a mean-field CRF over superpixel nodes with per-frame
+ * adjacency lists and node-to-node links between consecutive frames, for temporal smoothing of per-superpixel class
+ * probabilities.  Bit-identical to the reference's object code (g++ -O3 -mavx2 -mfma) with glibc's expf, logf and
+ * sqrtf.  Frames get times 0, 1, 2, ... from push_frame; the live ones always cover first_time..last_time.  Arrays of
+ * a frame are [C][N] float, clusters fslic_cluster[N] (y, x, r, g, b and num_members are read), adjacency lists CSR.
+ * All h_* buffers are host memory.  Every copy and kernel of a CRF runs on its stream: the last one passed to
+ * inference (NULL at first), which may be any stream, blocking or not.  inference, initialize and reset_inferred
+ * return at once; every other call synchronises that stream before it returns.  C * N must be < 2^31. */
+typedef struct fslic_crf fslic_crf;
+
+/* == SimpleCRFParams (simple-crf.h:11-19); defaults 10, 10, 13, 13, 80, 0, 3 */
+typedef struct fslic_crf_params {
+    float spatial_w, temporal_w, spatial_srgb, temporal_srgb, spatial_sxy, spatial_smooth_w, spatial_smooth_sxy;
+} fslic_crf_params;
+
+int fslic_b200_crf_create(int device, int num_classes, int num_nodes, fslic_crf** out);
+int fslic_b200_crf_destroy(fslic_crf* crf);
+int fslic_b200_crf_get_params(const fslic_crf* crf, fslic_crf_params* out);
+int fslic_b200_crf_set_params(fslic_crf* crf, const fslic_crf_params* params);
+/* first_time / last_time are -1 without frames; any pointer may be NULL */
+int fslic_b200_crf_times(const fslic_crf* crf, int* first_time, int* last_time, int* num_frames);
+int fslic_b200_crf_push_frame(fslic_crf* crf, int* time_out);
+int fslic_b200_crf_pop_frame(fslic_crf* crf, int* time_out); /* *time_out = -1 when there are no frames */
+
+/* Per frame; FSLIC_ENOFRAME when `time` is not live. */
+int fslic_b200_crf_set_clusters(fslic_crf* crf, int time, const fslic_cluster* h_clusters);
+int fslic_b200_crf_get_clusters(fslic_crf* crf, int time, fslic_cluster* h_out);
+/* Rows 0..num_rows-1 (num_rows <= N) get the lists h_neighbors[h_offsets[i] .. h_offsets[i+1]); the others keep
+ * theirs.  Neighbours outside [0, N) are refused and change nothing. */
+int fslic_b200_crf_set_connectivity(fslic_crf* crf, int time, int num_rows, const int32_t* h_offsets,
+                                    const int32_t* h_neighbors);
+/* h_offsets [N + 1]; h_neighbors (may be NULL) receives at most `cap` neighbours */
+int fslic_b200_crf_get_connectivity(fslic_crf* crf, int time, int32_t* h_offsets, int32_t* h_neighbors, long long cap);
+int fslic_b200_crf_set_unary(fslic_crf* crf, int time, const float* h_unary);
+int fslic_b200_crf_get_unary(fslic_crf* crf, int time, float* h_out);
+int fslic_b200_crf_set_unbiased(fslic_crf* crf, int time);                      /* logf(C) everywhere */
+int fslic_b200_crf_set_mask(fslic_crf* crf, int time, const int32_t* h_classes, float confidence); /* classes in [0,C) */
+int fslic_b200_crf_set_proba(fslic_crf* crf, int time, const float* h_proba);   /* -logf(p) */
+int fslic_b200_crf_get_inferred(fslic_crf* crf, int time, float* h_out);
+int fslic_b200_crf_reset_inferred(fslic_crf* crf, int time);                   /* q = expf(-unary) */
+int fslic_b200_crf_initialize(fslic_crf* crf);                                 /* reset_inferred on every frame */
+/* max_iter Jacobi mean-field steps over all frames: 1 + 2 max_iter kernel launches, no host synchronisation.
+ * FSLIC_ENOFRAME without frames (max_iter > 0). */
+int fslic_b200_crf_inference(fslic_crf* crf, unsigned long long max_iter, void* stream);
+int fslic_b200_crf_spatial_pairwise_energy(fslic_crf* crf, int time, int node_i, int node_j, float* out);
+/* node's energy between frame `time` of crf and frame `other_time` of `other` (may be crf), with crf's params */
+int fslic_b200_crf_temporal_pairwise_energy(fslic_crf* crf, int time, int node, fslic_crf* other, int other_time,
+                                            float* out);
+
+/* glibc's expf as the CRF evaluates it (fast_slic_b200/csrc/glibc_expf.cuh) over the bit patterns first,
+ * first + 1, ... (n values, wrapping at 2^32): the host compile into h_out, the device compile into d_out. */
+int fslic_b200_debug_expf_host(uint32_t first, long long n, float* h_out);
+int fslic_b200_debug_expf_device(int device, uint32_t first, long long n, float* d_out, void* stream);
 
 #ifdef __cplusplus
 }
