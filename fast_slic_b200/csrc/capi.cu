@@ -68,6 +68,21 @@ struct DeviceGuard {
             return set_err(FSLIC_ECUDA, std::string(#call) + ": " + cudaGetErrorString(e__));         \
     } while (0)
 
+// What the host enqueued for one assign pass (fslic_b200_debug_dispatch): kernel 5 = TMA-staged, 4 = LDG warp tiles,
+// 0 = generic, 10 / 11 / 12 = float-distance variant 0 / 1 / 2, 13 = preemptive, 14 = LSC, -1 = none yet.  Workers
+// are warps per CTA for the tile kernels and threads per CTA for the per-pixel ones; items are super tiles or pixels.
+struct PassDispatch {
+    int kernel = -1, tps = 0, grid = 0, workers = 0;
+    long long items = 0;
+    int trips = 0;  // ceil(items / (grid * workers)): rounds of the kernel's grid-stride walk
+};
+struct DispatchRecord {
+    PassDispatch upd, full;  // the last update pass launched, the full-assign pass
+    int prepare = 0;         // kernel of the last run_prepare: 3 = k_prepare3, 2 = k_prepare2, 1 = k_prepare
+    int fused = 0;           // update passes whose TMA tail ran the next pass's prepare
+    int lsc_trips = 0;       // rounds of k_lsc_features
+};
+
 struct fslic_ctx {
     int device = 0, H = 0, W = 0, K = 0, maxB = 0, S = 0, N = 0;
     bool cca_only = false;  // fslic_b200_create_cca: connectivity scratch only
@@ -165,7 +180,8 @@ struct fslic_ctx {
     std::vector<cudaEvent_t> lev;   // start / end events of each after_update launch (collect_timing)
     int lev_used = 0;
     int assign_impl = 5;       // 5: TMA-staged kernel where it applies (default), 4: always the LDG kernel (FSLIC_ASSIGN=4)
-    int last_assign_impl = 0;  // which kernel the last subsampled / full pass used (tests, bench)
+    DispatchRecord disp;       // launch decisions of the last iterate (tests, bench)
+    DispatchRecord gdisp;      // ... of the call captured into gexec: a replay makes the same ones
 };
 
 extern "C" const char* fslic_b200_last_error(void) { return g_err.c_str(); }
@@ -173,7 +189,31 @@ extern "C" const char* fslic_b200_version(void) { return "fast_slic_b200 0.1 (sm
 extern "C" int fslic_b200_sizeof_cluster(void) { return (int)sizeof(fslic_cluster); }
 extern "C" int fslic_b200_get_S(const fslic_ctx* ctx) { return ctx ? ctx->S : -1; }
 extern "C" int fslic_b200_launches_last_iterate(const fslic_ctx* ctx) { return ctx ? ctx->last_launches : -1; }
-extern "C" int fslic_b200_debug_assign_impl(const fslic_ctx* ctx) { return ctx ? ctx->last_assign_impl : -1; }
+extern "C" int fslic_b200_debug_assign_impl(const fslic_ctx* ctx) {
+    if (!ctx) return -1;
+    const int k = ctx->disp.full.kernel;
+    return k == 5 || k == 4 ? k : 0;
+}
+extern "C" int fslic_b200_debug_dispatch(const fslic_ctx* ctx, int32_t* out, int count) {
+    if (!ctx || !out) return set_err(FSLIC_EINVAL, "NULL argument");
+    const DispatchRecord& d = ctx->disp;
+    int32_t v[FSLIC_DISPATCH_COUNT];
+    int n = 0;
+    for (const PassDispatch* p : {&d.upd, &d.full}) {
+        v[n++] = p->kernel; v[n++] = p->tps; v[n++] = p->grid; v[n++] = p->workers;
+        v[n++] = (int32_t)std::min<long long>(p->items, INT32_MAX);
+        v[n++] = p->trips;
+    }
+    v[n++] = d.prepare; v[n++] = d.fused; v[n++] = d.lsc_trips;
+    for (int i = 0; i < count && i < FSLIC_DISPATCH_COUNT; i++) out[i] = v[i];
+    return FSLIC_OK;
+}
+static void record_pass(fslic_ctx* c, bool update, int kernel, int tps, long grid, int workers, long items) {
+    PassDispatch& d = update ? c->disp.upd : c->disp.full;
+    const long per_round = grid * workers;
+    d.kernel = kernel; d.tps = tps; d.grid = (int)grid; d.workers = workers; d.items = items;
+    d.trips = (int)((items + per_round - 1) / per_round);
+}
 extern "C" int fslic_b200_set_manhattan_spatial_dist(fslic_ctx* ctx, int on) {
     if (!ctx) return set_err(FSLIC_EINVAL, "NULL context");
     ctx->manhattan = on ? 1 : 0;
@@ -771,7 +811,7 @@ static int run_assign_pass(fslic_ctx* c, int batch, int stride, int rem, int cfg
         k_assign_preempt<true><<<(int)grid, 256, 0, st>>>(ap, SL_QUAD(c), SL_LABELS(c), SL_CINFO(c), SL_CELLS(c), d_clusters,
                                                           SL_ACC(c), c->pre_cellmap + (size_t)c->slice * ncell2, CW2, ncell2,
                                                           c->pre_nactive + c->slice);
-        c->last_assign_impl = 0;
+        record_pass(c, true, 13, 1, grid, 256, px);
         if (launches) *launches += 1;
         CK(cudaGetLastError());
         return FSLIC_OK;
@@ -795,7 +835,7 @@ static int run_assign_pass(fslic_ctx* c, int batch, int stride, int rem, int cfg
         else
             k_assign_lsc<false><<<(int)grid, 256, 0, st>>>(ap, SL_QUAD(c), SL_LABELS(c), SL_CINFO(c), SL_CELLS(c), c->lsc_feat,
                                                            c->lsc_cf, SL_ACC(c), c->lsc_box);
-        c->last_assign_impl = 0;
+        record_pass(c, update, 14, 1, grid, 256, px);
         if (launches) *launches += 1;
         CK(cudaGetLastError());
         return FSLIC_OK;
@@ -822,7 +862,7 @@ static int run_assign_pass(fslic_ctx* c, int batch, int stride, int rem, int cfg
         k_assign_real<V, false><<<(int)grid, 256, 0, st>>>(ap, SL_QUAD(c), SL_LABELS(c), SL_CINFO(c), SL_CELLS(c), cl, SL_ACC(c));
         if (variant == 0) { REAL_LAUNCH(0) } else if (variant == 1) { REAL_LAUNCH(1) } else { REAL_LAUNCH(2) }
 #undef REAL_LAUNCH
-        c->last_assign_impl = 0;
+        record_pass(c, update, 10 + variant, 1, grid, 256, px);
         if (launches) *launches += 1;
         CK(cudaGetLastError());
         return FSLIC_OK;
@@ -910,6 +950,7 @@ static int run_assign_pass(fslic_ctx* c, int batch, int stride, int rem, int cfg
                 ap.fuse_prepare = 1;
                 if (smem5 < tail_smem) smem5 = tail_smem;
                 *fused_out = true;
+                c->disp.fused++;
             }
             const assign5_fn fn = pick_assign5(g.TS, update, tps, ap.fuse_prepare != 0);
             long grid = (supers + warps5 - 1) / warps5;
@@ -940,13 +981,12 @@ static int run_assign_pass(fslic_ctx* c, int batch, int stride, int rem, int cfg
             fn<<<(int)grid, 32 * warps5, smem5, st>>>(ap, tmq, tml, qbase, lbase, SL_CINFO(c), SL_CELLS(c), SL_ACC(c), tbl,
                                                       fuse_clusters, SL_CINFO(c), SL_CELLS(c), c->prep_tickets + c->slice);
             if (e1) CK(cudaEventRecord(e1, st));
-            c->last_assign_impl = 5;
+            record_pass(c, update, 5, tps, grid, warps5, supers);
         }
     }
     if (use5) {
         // launched above
     } else if (g.fast) {
-        c->last_assign_impl = 4;
         const uint16_t* tbl = c->sptable + (update ? 0 : SPT_MAX_ELEMS);
         const assign_fn fn = pick_assign(g.TS, stride, update);
         int occ = 1;
@@ -971,11 +1011,12 @@ static int run_assign_pass(fslic_ctx* c, int batch, int stride, int rem, int cfg
         }
         fn<<<(int)grid, AS_THREADS, g.smem, st>>>(ap, SL_QUAD(c), SL_LABELS(c), SL_CINFO(c), SL_CELLS(c), SL_ACC(c), tbl);
         if (e1) CK(cudaEventRecord(e1, st));
+        record_pass(c, update, 4, ap.tps, grid, AS_WARPS, supers);
     } else {
-        c->last_assign_impl = 0;
         const long px = (long)ap.nsub * c->W * batch;
         long grid = (px + 255) / 256;
         if (grid > (long)c->num_sms * 64) grid = (long)c->num_sms * 64;
+        record_pass(c, update, 0, 1, grid, 256, px);
         if (update)
             k_assign_generic<true><<<(int)grid, 256, 0, st>>>(ap, SL_QUAD(c), SL_LABELS(c), SL_CINFO(c), SL_CELLS(c),
                                                               SL_ACC(c));
@@ -999,6 +1040,7 @@ static int run_prepare(fslic_ctx* c, fslic_cluster* d_clusters, int batch, int f
     if (preempt) {  // k_prepare carries the option's bookkeeping; after an update k_preempt_mark derives the active set
         k_prepare<<<batch, 1024, smem, st>>>(pp, d_clusters, SL_ACC(c), SL_QUAD(c), SL_CINFO(c), SL_CELLS(c),
                                              c->cinfo_tmp + (size_t)c->slice * c->K);
+        c->disp.prepare = 1;
         if (launches) *launches += 1;
         if (finalize && !last) {
             const int CW2 = ceil_div(c->W, 2 * c->S), ncell2 = CW2 * ceil_div(c->H, 2 * c->S);
@@ -1014,15 +1056,19 @@ static int run_prepare(fslic_ctx* c, fslic_cluster* d_clusters, int batch, int f
     // 0.412 vs 0.431 ms per blocking call); with a full batch its extra CTAs only contend (18 vs 13 us at 32 images)
     static const int forced = getenv("FSLIC_PREPARE") ? atoi(getenv("FSLIC_PREPARE")) : 0;
     const bool old_prepare = forced == 1 || (forced != 2 && batch >= 8);
-    if (forced != 1 && forced != 2 && c->K <= 1024 * PREP3_PER)
+    if (forced != 1 && forced != 2 && c->K <= 1024 * PREP3_PER) {
         k_prepare3<<<batch, 1024, smem, st>>>(pp, d_clusters, SL_ACC(c), SL_QUAD(c), SL_CINFO(c), SL_CELLS(c));
-    else if (old_prepare)
+        c->disp.prepare = 3;
+    } else if (old_prepare) {
         k_prepare<<<batch, 1024, smem, st>>>(pp, d_clusters, SL_ACC(c), SL_QUAD(c), SL_CINFO(c), SL_CELLS(c),
                                              c->cinfo_tmp + (size_t)c->slice * c->K);
-    else
+        c->disp.prepare = 1;
+    } else {
         k_prepare2<<<dim3(ceil_div(c->K, 256), batch), 256, smem, st>>>(
             pp, d_clusters, SL_ACC(c), SL_QUAD(c), SL_CINFO(c), SL_CELLS(c), c->cinfo_tmp + (size_t)c->slice * c->K,
             c->cell_cnt + (size_t)c->slice * (c->ncell + 1), c->prep_tickets + c->slice);
+        c->disp.prepare = 2;
+    }
     CK(cudaGetLastError());
     if (launches) *launches += 1;
     return FSLIC_OK;
@@ -1119,6 +1165,7 @@ static int lsc_before_iteration(fslic_ctx* c, const fslic_cluster* d_clusters, i
     long grid = (px + 255) / 256;
     if (grid > (long)c->num_sms * 32) grid = (long)c->num_sms * 32;
     k_lsc_features<<<(int)grid, 256, 0, st>>>(SL_QUAD(c), c->lsc_tab, c->H, c->W, batch, c->lsc_means, c->lsc_feat, c->lsc_w);
+    c->disp.lsc_trips = (int)((px + grid * 256 - 1) / (grid * 256));
     k_lsc_centroids<<<ceil_div(batch * c->K, 256), 256, 0, st>>>(c->lsc_feat, c->H, c->W, c->K, c->S, batch, d_clusters,
                                                                  c->lsc_cf, c->lsc_cf_init, c->lsc_box);
     if (launches) *launches += 3;
@@ -1217,6 +1264,7 @@ static int iterate_plain(fslic_ctx* c, const uint8_t* d_images, fslic_cluster* d
     USE_DEVICE(c->device);
     cudaStream_t st = (cudaStream_t)stream;
     int launches = 0;
+    c->disp = DispatchRecord();
     const bool timing = p->collect_timing != 0;
     c->kev_on = p->collect_timing >= 2;
     c->kev_used = 0;
@@ -1460,6 +1508,7 @@ static int iterate_graphed(fslic_ctx* c, const uint8_t* d_images, fslic_cluster*
         CK(cudaGraphLaunch(c->gexec, st));
         c->spt_valid = false;
         c->last_launches = c->glaunches;
+        c->disp = c->gdisp;
         return FSLIC_OK;
     }
     if (c->gexec) {
@@ -1488,6 +1537,7 @@ static int iterate_graphed(fslic_ctx* c, const uint8_t* d_images, fslic_cluster*
     }
     memcpy(&c->gkey, &k, sizeof(k));
     c->glaunches = c->last_launches;
+    c->gdisp = c->disp;
     CK(cudaGraphLaunch(c->gexec, st));
     c->spt_valid = false;
     return FSLIC_OK;
@@ -1508,6 +1558,7 @@ static int iterate_host_enqueue_body(fslic_ctx* c, const uint8_t* h_images, fsli
         CK(cudaStreamSynchronize(c->own_stream));
         c->pending = false;
     }
+    c->disp = DispatchRecord();
     // Software pipeline over chunks of the batch: H2D(chunk i+1) | compute(chunk i) | D2H(chunk i-1) on three
     // streams, so for batches the PCIe copies hide behind the kernels (and vice versa).  With pinned host
     // buffers the copies are truly asynchronous; pageable buffers still work, just without overlap.

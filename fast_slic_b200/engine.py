@@ -255,5 +255,21 @@ class Engine:
         """5: TMA-staged assign kernel, 4: LDG kernel, 0: brute force (last pass of the last iterate)."""
         return int(self._L.fslic_b200_debug_assign_impl(self._h))
 
+    DISPATCH_KERNELS = {5: "tma", 4: "ldg", 0: "generic", 10: "real_standard", 11: "real_l2", 12: "real_noq",
+                        13: "preemptive", 14: "lsc", -1: None}
+    PREPARE_KERNELS = {3: "k_prepare3", 2: "k_prepare2", 1: "k_prepare", 0: None}
+
+    def dispatch(self):
+        """Launch decisions of the last iterate (fslic_b200_debug_dispatch), as the host made them:
+        {"update": pass, "full": pass, "prepare": int, "fused_prepares": int, "lsc_features_trips": int}, a pass being
+        {"kernel", "tps", "grid", "workers", "items", "trips"} (kernel codes in DISPATCH_KERNELS, prepare codes in
+        PREPARE_KERNELS).  "update" is the last update pass launched, "full" the full-assign pass."""
+        out = (C.c_int32 * _lib.DISPATCH_COUNT)()
+        check(self._L.fslic_b200_debug_dispatch(self._h, out, _lib.DISPATCH_COUNT))
+        v = [int(x) for x in out]
+        n = len(_lib.PASS_FIELDS)
+        return {"update": dict(zip(_lib.PASS_FIELDS, v[:n])), "full": dict(zip(_lib.PASS_FIELDS, v[n:2 * n])),
+                "prepare": v[2 * n], "fused_prepares": v[2 * n + 1], "lsc_features_trips": v[2 * n + 2]}
+
     def launches_last_iterate(self):
         return int(self._L.fslic_b200_launches_last_iterate(self._h))

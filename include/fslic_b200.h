@@ -213,6 +213,21 @@ int fslic_b200_launches_last_iterate(const fslic_ctx* ctx);
  * by the environment variable FSLIC_ASSIGN=4 at context creation), 0: the brute-force kernel / none yet. */
 int fslic_b200_debug_assign_impl(const fslic_ctx* ctx);
 
+/* Diagnostics: the launch decisions of the last iterate (any iterate entry point, host or device), as the host made
+ * them when it enqueued the work -- no device synchronisation.  Writes min(count, FSLIC_DISPATCH_COUNT) int32 values:
+ *   [0..5]   the last update pass launched: kernel, tps, grid, workers, items, trips
+ *   [6..11]  the full-assign pass: the same six values
+ *   [12]     kernel of the last prepare launch: 3 = k_prepare3, 2 = k_prepare2, 1 = k_prepare, 0 = none
+ *   [13]     update passes whose TMA tail ran the next pass's prepare
+ *   [14]     rounds of the LSC feature kernel (0 outside LSC)
+ * kernel: 5 = TMA-staged, 4 = LDG warp tiles, 0 = generic, 10 / 11 / 12 = float-distance variant 0 / 1 / 2,
+ * 13 = preemptive, 14 = LSC, -1 = no such pass.  tps: warp tiles per super tile (1 for the per-pixel kernels).
+ * grid: CTAs launched.  workers: warps per CTA (tile kernels) or threads per CTA (per-pixel kernels).  items: super
+ * tiles or pixels of the pass over the batch slice it ran on.  trips: ceil(items / (grid * workers)), the rounds of the
+ * grid-stride walk.  The blocking host entry point may run a batch as two halves: the values are the second half's. */
+#define FSLIC_DISPATCH_COUNT 15
+int fslic_b200_debug_dispatch(const fslic_ctx* ctx, int32_t* out, int count);
+
 /* ---- SimpleCRF (src/simple-crf.{h,hpp,cpp}, csimple_crf.pyx): a mean-field CRF over superpixel nodes with per-frame
  * adjacency lists and node-to-node links between consecutive frames, for temporal smoothing of per-superpixel class
  * probabilities.  Bit-identical to the reference's object code (g++ -O3 -mavx2 -mfma) with glibc's expf, logf and

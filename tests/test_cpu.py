@@ -172,6 +172,18 @@ def test_abi_library_exports_every_declared_symbol():
     assert L.fslic_b200_version().startswith(b"fast_slic_b200")
 
 
+def test_abi_declares_the_dispatch_read_back():
+    from fast_slic_b200 import _lib
+    L = _lib.lib()
+    assert "fslic_b200_debug_dispatch" in _lib.EXPORTED_SYMBOLS
+    assert hasattr(L, "fslic_b200_debug_dispatch")
+    assert L.fslic_b200_debug_dispatch.argtypes is not None  # bound: a pointer argument must not be passed as a C int
+    header = open(os.path.join(ROOT, "include", "fslic_b200.h")).read()
+    assert "int fslic_b200_debug_dispatch(const fslic_ctx* ctx, int32_t* out, int count);" in header
+    assert re.search(r"#define FSLIC_DISPATCH_COUNT (\d+)", header).group(1) == str(_lib.DISPATCH_COUNT)
+    assert _lib.DISPATCH_COUNT == 2 * len(_lib.PASS_FIELDS) + 3
+
+
 def test_abi_is_sm90a_only():
     out = subprocess.run(["cuobjdump", "--list-elf", os.path.join(ROOT, "fast_slic_b200", "libfslic_b200.so")],
                          capture_output=True, text=True).stdout
