@@ -17,7 +17,7 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_rgb_to_quad", "fslic_b200_debug_heap_select", "fslic_b200_stage_ms", "fslic_b200_get_S",
     "fslic_b200_launches_last_iterate", "fslic_b200_assign_kernel_time", "fslic_b200_debug_cca_counters", "fslic_b200_debug_select_profile",
     "fslic_b200_iterate_host_async", "fslic_b200_wait", "fslic_b200_create_cca",
-    "fslic_b200_debug_assign_impl", "fslic_b200_debug_dispatch", "fslic_b200_connectivity_scratch_bytes", "fslic_b200_get_connectivity",
+    "fslic_b200_debug_assign_impl", "fslic_b200_debug_dispatch", "fslic_b200_debug_cca_dispatch", "fslic_b200_connectivity_scratch_bytes", "fslic_b200_get_connectivity",
     "fslic_b200_get_mask_density", "fslic_b200_cluster_density_to_mask", "fslic_b200_cca_stage_ms",
     "fslic_b200_iterate_real", "fslic_b200_iterate_preemptive", "fslic_b200_set_manhattan_spatial_dist",
     "fslic_b200_iterate_lsc", "fslic_b200_debug_lsc_stages",
@@ -34,6 +34,8 @@ STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_
 LSC_STAGE_NAMES = ("before_iteration", "after_update")  # FSLIC_T_BEFORE_ITERATION, FSLIC_T_AFTER_UPDATE
 DISPATCH_COUNT = 15  # FSLIC_DISPATCH_COUNT
 PASS_FIELDS = ("kernel", "tps", "grid", "workers", "items", "trips")  # one pass of fslic_b200_debug_dispatch
+CCA_DISPATCH_FIELDS = ("heap_smem", "heap_smem_max_k", "sub_batches", "split", "number_nb")  # fslic_b200_debug_cca_dispatch
+CCA_DISPATCH_COUNT = len(CCA_DISPATCH_FIELDS)  # FSLIC_CCA_DISPATCH_COUNT
 CCA_STAGE_NAMES =("build_disjoint_set", "flatten", "threshold_by_area", "sort", "substitute", "output")  # cca.cpp:194-263
 
 
@@ -93,6 +95,7 @@ def lib():
     L.fslic_b200_launches_last_iterate.argtypes = [vp]
     L.fslic_b200_debug_assign_impl.argtypes = [vp]
     L.fslic_b200_debug_dispatch.argtypes = [vp, C.POINTER(C.c_int32), i32]
+    L.fslic_b200_debug_cca_dispatch.argtypes = [vp, C.POINTER(C.c_int32), i32]
     L.fslic_b200_connectivity_scratch_bytes.argtypes = [i32]
     L.fslic_b200_connectivity_scratch_bytes.restype = C.c_size_t
     L.fslic_b200_get_connectivity.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, C.c_size_t, vp]

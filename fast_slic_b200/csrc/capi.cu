@@ -81,6 +81,12 @@ struct DispatchRecord {
     int prepare = 0;         // kernel of the last run_prepare: 3 = k_prepare3, 2 = k_prepare2, 1 = k_prepare
     int fused = 0;           // update passes whose TMA tail ran the next pass's prepare
     int lsc_trips = 0;       // rounds of k_lsc_features
+    // connectivity stage (run_cca), recorded when enqueued
+    int cca_heap_smem = -1;       // k_cca_select's heap: 1 = shared memory, 0 = global memory, -1 = no connectivity stage ran
+    int cca_heap_smem_max_k = 0;  // largest K whose heap fits shared memory on this device
+    int cca_sub_batches = 0;      // sub-batches of at most cca_batch images
+    int cca_split = 0;            // first sub-batch: settled images' tail on the side stream (nb >= 4)
+    int cca_number_nb = 0;        // first sub-batch: 1024-pixel blocks per k_ccl_number warp
 };
 
 struct fslic_ctx {
@@ -206,6 +212,14 @@ extern "C" int fslic_b200_debug_dispatch(const fslic_ctx* ctx, int32_t* out, int
     }
     v[n++] = d.prepare; v[n++] = d.fused; v[n++] = d.lsc_trips;
     for (int i = 0; i < count && i < FSLIC_DISPATCH_COUNT; i++) out[i] = v[i];
+    return FSLIC_OK;
+}
+extern "C" int fslic_b200_debug_cca_dispatch(const fslic_ctx* ctx, int32_t* out, int count) {
+    if (!ctx || !out) return set_err(FSLIC_EINVAL, "NULL argument");
+    const DispatchRecord& d = ctx->disp;
+    const int32_t v[FSLIC_CCA_DISPATCH_COUNT] = {d.cca_heap_smem, d.cca_heap_smem_max_k, d.cca_sub_batches, d.cca_split,
+                                                 d.cca_number_nb};
+    for (int i = 0; i < count && i < FSLIC_CCA_DISPATCH_COUNT; i++) out[i] = v[i];
     return FSLIC_OK;
 }
 static void record_pass(fslic_ctx* c, bool update, int kernel, int tps, long grid, int workers, long items) {
@@ -524,6 +538,10 @@ static int run_cca(fslic_ctx* c, const uint16_t* d_in, uint16_t* d_out, int batc
     static const int sel_sync = (getenv("FSLIC_SELSYNC") && atoi(getenv("FSLIC_SELSYNC")) == 0) ? 0 : 1;
     cp.sel_sync = sel_sync;
     if (K + 2 > c->heap_K) return set_err(FSLIC_EINVAL, "K too large for the selection heap");
+    c->disp.cca_heap_smem = cp.heap_in_smem ? 1 : 0;
+    c->disp.cca_heap_smem_max_k =
+        (int)std::max<long>(0, ((long)c->max_smem_optin - 8 * 1024 - SEL_CHUNK * 8) / 8 / 2 - 2);  // (2K+4)*8 fits
+    c->disp.cca_sub_batches = ceil_div(batch, c->cca_batch);
     for (int b0 = 0; b0 < batch; b0 += c->cca_batch) {
         const int nb = (batch - b0 < c->cca_batch) ? (batch - b0) : c->cca_batch;
         const uint16_t* in = d_in + (size_t)b0 * N;
@@ -553,6 +571,10 @@ static int run_cca(fslic_ctx* c, const uint16_t* d_in, uint16_t* d_out, int batc
         // grids of the per-component walks: sized for full batches (a few CTAs per image); a small batch gets more
         // CTAs per image instead, it is all dependent-load latency there
         const int number_grid = nb >= 8 ? CCA_NUMBER_GRID : std::min(std::max(ceil_div(cp.nblk, 32), CCA_NUMBER_GRID), 64);
+        if (b0 == 0) {
+            c->disp.cca_split = nb >= 4;
+            c->disp.cca_number_nb = ceil_div(cp.nblk, number_grid * (CCA_BLOCK / 32));  // NB of k_ccl_number
+        }
         k_ccl_number<<<dim3(number_grid, nb), CCA_BLOCK, 0, st>>>(cp, x_rootbuf, x_aux, x_blkcnt, x_blkoff, x_cleader, x_carea,
                                                                       x_counters, x_ahist);
         if (timed) CK(cudaEventRecord(c->cev[2], st));
@@ -641,6 +663,7 @@ extern "C" int fslic_b200_enforce_connectivity(fslic_ctx* c, uint16_t* d_labels,
     if (K <= 0) return FSLIC_OK;  // context.cpp:17
     if (K > 65535) return set_err(FSLIC_EINVAL, "K must fit the u16 label type");
     USE_DEVICE(c->device);
+    c->disp = DispatchRecord();
     return run_cca(c, d_labels, d_labels, batch, K, min_threshold, (cudaStream_t)stream, nullptr);
 }
 

@@ -263,13 +263,18 @@ class Engine:
         """Launch decisions of the last iterate (fslic_b200_debug_dispatch), as the host made them:
         {"update": pass, "full": pass, "prepare": int, "fused_prepares": int, "lsc_features_trips": int}, a pass being
         {"kernel", "tps", "grid", "workers", "items", "trips"} (kernel codes in DISPATCH_KERNELS, prepare codes in
-        PREPARE_KERNELS).  "update" is the last update pass launched, "full" the full-assign pass."""
+        PREPARE_KERNELS).  "update" is the last update pass launched, "full" the full-assign pass.  "cca" holds the
+        connectivity stage's decisions of the last iterate or enforce_connectivity (fslic_b200_debug_cca_dispatch),
+        {name: value} over _lib.CCA_DISPATCH_FIELDS (heap_smem -1 when no connectivity stage ran)."""
         out = (C.c_int32 * _lib.DISPATCH_COUNT)()
         check(self._L.fslic_b200_debug_dispatch(self._h, out, _lib.DISPATCH_COUNT))
         v = [int(x) for x in out]
+        cca = (C.c_int32 * _lib.CCA_DISPATCH_COUNT)()
+        check(self._L.fslic_b200_debug_cca_dispatch(self._h, cca, _lib.CCA_DISPATCH_COUNT))
         n = len(_lib.PASS_FIELDS)
         return {"update": dict(zip(_lib.PASS_FIELDS, v[:n])), "full": dict(zip(_lib.PASS_FIELDS, v[n:2 * n])),
-                "prepare": v[2 * n], "fused_prepares": v[2 * n + 1], "lsc_features_trips": v[2 * n + 2]}
+                "prepare": v[2 * n], "fused_prepares": v[2 * n + 1], "lsc_features_trips": v[2 * n + 2],
+                "cca": dict(zip(_lib.CCA_DISPATCH_FIELDS, [int(x) for x in cca]))}
 
     def launches_last_iterate(self):
         return int(self._L.fslic_b200_launches_last_iterate(self._h))

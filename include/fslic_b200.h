@@ -228,6 +228,18 @@ int fslic_b200_debug_assign_impl(const fslic_ctx* ctx);
 #define FSLIC_DISPATCH_COUNT 15
 int fslic_b200_debug_dispatch(const fslic_ctx* ctx, int32_t* out, int count);
 
+/* Diagnostics: the launch decisions of the connectivity stage of the last iterate (any entry point) or
+ * fslic_b200_enforce_connectivity call, as the host made them when it enqueued the work -- no device synchronisation.
+ * Writes min(count, FSLIC_CCA_DISPATCH_COUNT) int32 values:
+ *   [0]  heap_smem: the std::partial_sort replay's heap in shared memory (1) or in global memory (0); -1 = no
+ *        connectivity stage ran.  Decided per call from K, whether or not an image then needs the replay
+ *   [1]  heap_smem_max_k: the largest K whose heap fits shared memory on this device
+ *   [2]  sub_batches: sub-batches the batch ran in (the context's scratch holds a bounded number of images)
+ *   [3]  split: the first sub-batch ran its settled images' tail on a side stream (4 or more images)
+ *   [4]  number_nb: 1024-pixel blocks per warp of the component-numbering kernel, first sub-batch */
+#define FSLIC_CCA_DISPATCH_COUNT 5
+int fslic_b200_debug_cca_dispatch(const fslic_ctx* ctx, int32_t* out, int count);
+
 /* ---- SimpleCRF (src/simple-crf.{h,hpp,cpp}, csimple_crf.pyx): a mean-field CRF over superpixel nodes with per-frame
  * adjacency lists and node-to-node links between consecutive frames, for temporal smoothing of per-superpixel class
  * probabilities.  Bit-identical to the reference's object code (g++ -O3 -mavx2 -mfma) with glibc's expf, logf and

@@ -93,7 +93,8 @@ BIG_CASES = [
     ("B_1280x720_K1600_msf.1_s40", "syn", 720, 1280, 1600, dict(min_size_factor=0.1, sigma=40.0)),
     ("C_1920x1080_K2000_msf0", "syn", 1080, 1920, 2000, dict(min_size_factor=0.0)),
     ("D_3840x2160_K4000_msf0", "tiled", 2160, 3840, 4000, dict(min_size_factor=0.0)),
-    # > 2^24 pixels: more than 32 of the 1024-pixel blocks per numbering warp (k_ccl_number's outer chunk loop)
+    # > 2^24 pixels, a single image: k_ccl_number gets 64 CTAs, so 9 blocks per numbering warp and one trip of its
+    # outer chunk loop (the second trip needs 8+ images above 16.7 M px: tests/test_cca_gpu.py)
     ("huge_4100x4200_K3000_msf.1", "tiled", 4100, 4200, 3000, dict(min_size_factor=0.1, sigma=20.0)),
 ]
 
