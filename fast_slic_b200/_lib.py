@@ -28,6 +28,8 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_crf_set_proba", "fslic_b200_crf_get_inferred", "fslic_b200_crf_reset_inferred",
     "fslic_b200_crf_initialize", "fslic_b200_crf_inference", "fslic_b200_crf_spatial_pairwise_energy",
     "fslic_b200_crf_temporal_pairwise_energy", "fslic_b200_debug_expf_host", "fslic_b200_debug_expf_device",
+    "fslic_b200_set_trace", "fslic_b200_trace_info", "fslic_b200_trace_snapshots", "fslic_b200_format_report",
+    "fslic_b200_free_report", "fslic_b200_debug_graph_counts",
 )
 
 STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity", "iterate")
@@ -104,6 +106,14 @@ def lib():
     L.fslic_b200_assign_kernel_time.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]
     L.fslic_b200_debug_cca_counters.argtypes = [vp, C.POINTER(C.c_int32), i32]
     L.fslic_b200_debug_select_profile.argtypes = [vp, C.POINTER(C.c_longlong), i32]
+    L.fslic_b200_set_trace.argtypes = [vp, i32]
+    L.fslic_b200_debug_graph_counts.argtypes = [vp, C.POINTER(i32), C.POINTER(i32)]
+    L.fslic_b200_trace_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
+    L.fslic_b200_trace_snapshots.argtypes = [vp, i32, vp, vp, vp, C.POINTER(C.c_uint32)]
+    L.fslic_b200_format_report.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, C.POINTER(C.c_void_p),
+                                           C.POINTER(C.c_size_t)]
+    L.fslic_b200_free_report.argtypes = [vp]
+    L.fslic_b200_free_report.restype = None
     assert L.fslic_b200_sizeof_cluster() == 32
     _lib = L
     return L
@@ -117,3 +127,27 @@ def check(rc):
         if rc == -3:
             raise MemoryError(msg)
         raise FslicError("fslic_b200 error %d: %s" % (rc, msg))
+
+
+def format_recorder_report(H, W, assignment, min_dists, clusters):
+    """The reference's debug_mode report (recorder.h) as bytes, from snapshot arrays laid out like
+    Engine.trace_snapshots returns them: assignment u16[T, H*W], min_dists u16 or float32 [T, H*W], clusters [T, K]
+    32-byte records.  Formatted by fslic_b200_format_report (host code, no device needed)."""
+    import numpy as np
+    assignment = np.ascontiguousarray(assignment, np.uint16)
+    min_dists = np.ascontiguousarray(min_dists)
+    clusters = np.ascontiguousarray(clusters)
+    if min_dists.dtype not in (np.uint16, np.float32):
+        raise ValueError("min_dists must be uint16 or float32")
+    T = clusters.shape[0] if clusters.ndim == 2 else 0
+    K = clusters.shape[1] if clusters.ndim == 2 else 0
+    if clusters.dtype.itemsize != 32 or assignment.size != T * H * W or min_dists.size != T * H * W:
+        raise ValueError("snapshot arrays do not match T=%d, H=%d, W=%d" % (T, H, W))
+    L = lib()
+    out, n = C.c_void_p(), C.c_size_t()
+    check(L.fslic_b200_format_report(int(H), int(W), K, T, int(min_dists.dtype == np.float32), assignment.ctypes.data,
+                                     min_dists.ctypes.data, clusters.ctypes.data, C.byref(out), C.byref(n)))
+    try:
+        return C.string_at(out, n.value)
+    finally:
+        L.fslic_b200_free_report(out)

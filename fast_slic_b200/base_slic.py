@@ -17,6 +17,8 @@ from . import _lib
 from .engine import CLUSTER_DTYPE, Engine, require_cuda
 
 ARCH_NAME = "cuda/sm_90a"
+# last_recorder_report of a call without debug_mode (the reference's would also carry height and width)
+EMPTY_RECORDER_REPORT = b'{"snapshots":[]}'
 _SUPPORTED_ARCHS = (ARCH_NAME,)
 
 # Contexts are cached and reused (the reference rebuilds one per call, cfast_slic.pyx:171-197), in a small LRU:
@@ -208,6 +210,10 @@ class SlicModel(object):
         if self.preemptive and self.real_dist:
             raise NotImplementedError("preemptive=True together with a float-distance variant is outside the CUDA hot path")
 
+    def _traced(self):
+        """debug_mode records the reference's snapshots (recorder.h); without it the report stays EMPTY_RECORDER_REPORT."""
+        return bool(self.debug_mode)
+
     def initialize(self, image):
         """cfast_slic.pyx:124-147."""
         image = _check_image(image)
@@ -227,7 +233,7 @@ class SlicModel(object):
         H, W, _ = image.shape
         params = Engine.params(compactness, min_size_factor, subsample_stride, self.convert_to_lab, max_iter,
                                collect_timing=1)
-        if self.real_dist or self.preemptive:
+        if self.real_dist or self.preemptive or self._traced():
             return self._iterate_real_dist(image, params)
         clusters = np.ascontiguousarray(self._clusters)[None]
         # the lock covers the timing read-out too: it belongs to this call, not to another thread's next one
@@ -247,27 +253,40 @@ class SlicModel(object):
             node("enforce_connectivity", ms["enforce_connectivity"],
                  [node("cca", ms["enforce_connectivity"], [node(n, cca[n]) for n in _lib.CCA_STAGE_NAMES])]),
         ]))
-        self.last_recorder_report = b'{"snapshots":[]}'
+        self.last_recorder_report = EMPTY_RECORDER_REPORT
         return labels[0]
 
 
 def _iterate_real_dist(self, image, params):
     """cfast_slic.pyx:198-252: the float-distance contexts (fslic_b200_iterate_real), LSC (fslic_b200_iterate_lsc) and
-    the `preemptive` option (fslic_b200_iterate_preemptive), all through device buffers."""
+    the `preemptive` option (fslic_b200_iterate_preemptive), all through device buffers; also the default contexts
+    (fslic_b200_iterate) when debug_mode records snapshots, which only the device entry points do."""
     H, W, _ = image.shape
+    traced = self._traced()
+    report = EMPTY_RECORDER_REPORT
     with _locked(lambda: get_engine(H, W, self._num_components, 1, self.device)) as eng:
         with torch.cuda.device(eng.device):
             img = torch.from_numpy(image).to(eng.device)[None]
             cl = torch.from_numpy(np.ascontiguousarray(self._clusters).view(np.uint8).reshape(1, -1, 32).copy()).to(eng.device)
             spatial = dict(manhattan_spatial_dist=self.manhattan_spatial_dist)  # cfast_slic.pyx:186,246
-            if self.preemptive:  # cfast_slic.pyx:183-184
-                labels = eng.iterate_preemptive(img, cl, params, self.preemptive_thres, **spatial)
-            elif self.real_dist_type == "lsc":  # cfast_slic.pyx:207-214
-                labels = eng.iterate_lsc(img, cl, params, **spatial)
-            else:
-                labels = eng.iterate_real(self.real_dist_type, img, cl, params, **spatial)
+            if traced:
+                eng.set_trace(True)
+            try:
+                if self.preemptive:  # cfast_slic.pyx:183-184
+                    labels = eng.iterate_preemptive(img, cl, params, self.preemptive_thres, **spatial)
+                elif not self.real_dist:  # cfast_slic.pyx:170-196
+                    labels = eng.iterate(img, cl, params, **spatial)
+                elif self.real_dist_type == "lsc":  # cfast_slic.pyx:207-214
+                    labels = eng.iterate_lsc(img, cl, params, **spatial)
+                else:
+                    labels = eng.iterate_real(self.real_dist_type, img, cl, params, **spatial)
+            finally:
+                if traced:
+                    eng.set_trace(False)
             ms = eng.stage_ms()
             ms.update(eng.lsc_stage_ms())
+            if traced:  # cfast_slic.pyx:196,256
+                report = eng.recorder_report(0)
             self._clusters = cl[0].cpu().numpy().view(CLUSTER_DTYPE).reshape(-1)
             out = labels[0].cpu().numpy()
     # the reference's fstimer tree (context.cpp:112-192); LSC adds its two hooks in their places (:152, :170)
@@ -278,7 +297,7 @@ def _iterate_real_dist(self, image, params):
     self.last_timing_report = json.dumps({
         "name": "iterate", "duration": int(ms["iterate"] * 1000),
         "children": [{"name": n, "duration": int(ms[n] * 1000), "children": []} for n in names]})
-    self.last_recorder_report = b'{"snapshots":[]}'
+    self.last_recorder_report = report
     return out
 
 

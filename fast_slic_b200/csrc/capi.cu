@@ -23,6 +23,8 @@
 #include "cca.cuh"
 #include "common.cuh"
 #include "lab.cuh"
+#include "trace.cuh"
+#include "recorder_format.h"
 
 #define SPT_MAX_ELEMS (128 * 1024)  // u16 elements per spatial patch buffer
 
@@ -164,6 +166,7 @@ struct fslic_ctx {
         int manhattan;
     } gkey = {nullptr, nullptr, nullptr, 0, {0.f, 0.f, 0, 0, 0, 0}, 0}, gkey_seen = {nullptr, nullptr, nullptr, 0, {0.f, 0.f, 0, 0, 0, 0}, 0};
     int glaunches = 0;
+    int graph_captures = 0, graph_replays = 0;  // fslic_b200_debug_graph_counts
     float assign_kernel_ms = 0.f;
     int assign_kernel_launches = 0;
     bool spt_valid = false, spt_has_sub = false;  // what c->sptable currently holds (build_patches)
@@ -188,6 +191,12 @@ struct fslic_ctx {
     int assign_impl = 5;       // 5: TMA-staged kernel where it applies (default), 4: always the LDG kernel (FSLIC_ASSIGN=4)
     DispatchRecord disp;       // launch decisions of the last iterate (tests, bench)
     DispatchRecord gdisp;      // ... of the call captured into gexec: a replay makes the same ones
+    // debug_mode (fslic_b200_set_trace, trace.cuh): snapshots of the last traced iterate, [B][T] slots, allocated on demand
+    bool trace_on = false;
+    int tr_T = 0, tr_B = 0, tr_dist_bytes = 0;  // what the buffers hold (tr_T == 0: nothing recorded)
+    size_t tr_cap = 0;                          // bytes allocated at tr_buf
+    void* tr_buf = nullptr;                     // clusters [B][T][K], then assignment [B][T][N], then min_dists [B][T][N]
+    unsigned int* tr_bad = nullptr;             // pixels whose label disagreed with the trace kernel's argmin
 };
 
 extern "C" const char* fslic_b200_last_error(void) { return g_err.c_str(); }
@@ -294,7 +303,7 @@ extern "C" int fslic_b200_destroy(fslic_ctx* c) {
     if (c->pre_nactive) cudaFree(c->pre_nactive);
     for (auto& e : c->pipe_ev) cudaEventDestroy(e);
     for (void* p : {(void*)c->lsc_feat, (void*)c->lsc_w, (void*)c->lsc_tab, (void*)c->lsc_means, (void*)c->lsc_cf,
-                    (void*)c->lsc_cf_init, (void*)c->lsc_box})
+                    (void*)c->lsc_cf_init, (void*)c->lsc_box, c->tr_buf, (void*)c->tr_bad})
         if (p) cudaFree(p);
     for (auto& e : c->lev) cudaEventDestroy(e);
     delete c;
@@ -1216,6 +1225,103 @@ static int lsc_after_update(fslic_ctx* c, int batch, int stride, cudaStream_t st
     return FSLIC_OK;
 }
 
+// ---- debug_mode tracing (trace.cuh) -------------------------------------------------------------------------------
+// Snapshot s of image b (s = 0 is the reference's iteration -1, s = i + 1 its iteration i) lives in slot b * T + s of
+// three regions of one allocation: clusters [B][T][K], min_dists [B][T][N] (u16 or float), assignment [B][T][N].
+static fslic_cluster* tr_clusters(const fslic_ctx* c) { return static_cast<fslic_cluster*>(c->tr_buf); }
+static char* tr_dist(const fslic_ctx* c) {
+    return static_cast<char*>(c->tr_buf) + (size_t)c->tr_B * c->tr_T * c->K * sizeof(fslic_cluster);
+}
+static uint16_t* tr_assign(const fslic_ctx* c) {
+    return reinterpret_cast<uint16_t*>(tr_dist(c) + (size_t)c->tr_B * c->tr_T * c->N * c->tr_dist_bytes);
+}
+
+// Sizes the snapshot buffers for this call (they grow, never shrink) and clears the self-check counter.
+static int trace_begin(fslic_ctx* c, int batch, int max_iter, int variant, cudaStream_t st) {
+    c->tr_T = 0;
+    const int T = max_iter + 1, db = (variant >= 0 && variant <= 2) || variant == 4 ? 4 : 2;  // float contexts: float distances
+    const size_t need = (size_t)T * batch * ((size_t)c->K * sizeof(fslic_cluster) + (size_t)c->N * (2 + db));
+    if (!c->tr_bad && cudaMalloc(reinterpret_cast<void**>(&c->tr_bad), sizeof(unsigned int)) != cudaSuccess) {
+        c->tr_bad = nullptr;
+        cudaGetLastError();
+        return set_err(FSLIC_ENOMEM, "out of device memory (trace counter)");
+    }
+    if (need > c->tr_cap) {
+        if (c->tr_buf) cudaFree(c->tr_buf);
+        c->tr_buf = nullptr;
+        c->tr_cap = 0;
+        if (cudaMalloc(&c->tr_buf, need) != cudaSuccess) {
+            c->tr_buf = nullptr;
+            cudaGetLastError();
+            return set_err(FSLIC_ENOMEM, "out of device memory (" + std::to_string(need >> 20) + " MiB of debug_mode snapshots)");
+        }
+        c->tr_cap = need;
+    }
+    c->tr_T = T;
+    c->tr_B = batch;
+    c->tr_dist_bytes = db;
+    CK(cudaMemsetAsync(c->tr_bad, 0, sizeof(unsigned int), st));
+    return FSLIC_OK;
+}
+
+// Snapshot -1: assignment all 0xFFFF (context.cpp:140-145), min_dists all 0 (a fresh context's calloc'd array,
+// simd-helper.hpp:65), the cluster records of k_trace_seed.
+static int trace_seed(fslic_ctx* c, const fslic_cluster* d_clusters, int batch, cudaStream_t st, int* launches) {
+    const size_t N = c->N, T = c->tr_T;
+    k_trace_seed<<<ceil_div(batch * c->K, 256), 256, 0, st>>>(c->H, c->W, c->K, batch, SL_QUAD(c), d_clusters, tr_clusters(c),
+                                                             (long long)T * c->K);
+    CK(cudaGetLastError());
+    CK(cudaMemset2DAsync(tr_assign(c), T * N * 2, 0xFF, N * 2, batch, st));
+    CK(cudaMemset2DAsync(tr_dist(c), T * N * c->tr_dist_bytes, 0, N * c->tr_dist_bytes, batch, st));
+    (*launches)++;
+    return FSLIC_OK;
+}
+
+// Assignment and minimum distances after update pass `it` (slot it + 1), from the records that pass read.  Runs before
+// the next prepare rewrites them and, for LSC, before after_update.
+static int trace_pass(fslic_ctx* c, int batch, int it, int stride, int rem, float coef, int variant,
+                      const fslic_cluster* d_clusters, cudaStream_t st, int* launches) {
+    TraceParams tp;
+    memset(&tp, 0, sizeof(tp));
+    AssignParams& ap = tp.ap;
+    ap.H = c->H; ap.W = c->W; ap.K = c->K; ap.S = c->S; ap.B = batch;
+    ap.stride = stride; ap.rem = rem; ap.cfg_stride = stride;
+    ap.G = c->G; ap.cellW = c->cellW; ap.cellH = c->cellH; ap.ncell = c->ncell;
+    ap.coef = coef;
+    ap.manhattan = c->manhattan;
+    tp.fresh_after = it + 1;
+    tp.preempt = variant == 3;
+    tp.img_pitch = (long long)c->tr_T * c->N;
+    tp.feat = c->lsc_feat;
+    tp.cf = c->lsc_cf;
+    const size_t slot = (size_t)(it + 1) * c->N;
+    uint16_t* oa = tr_assign(c) + slot;
+    void* od = tr_dist(c) + slot * c->tr_dist_bytes;
+    const long px = (long)c->N * batch;
+    long grid = (px + 255) / 256;
+    if (grid > (long)c->num_sms * 32) grid = (long)c->num_sms * 32;
+#define TRACE_LAUNCH(KIND) \
+    k_trace_pass<KIND><<<(int)grid, 256, 0, st>>>(tp, SL_QUAD(c), SL_LABELS(c), SL_CINFO(c), SL_CELLS(c), d_clusters, oa, od, c->tr_bad)
+    if (variant == 0) TRACE_LAUNCH(0);
+    else if (variant == 1) TRACE_LAUNCH(1);
+    else if (variant == 2) TRACE_LAUNCH(2);
+    else if (variant == 4) TRACE_LAUNCH(4);
+    else TRACE_LAUNCH(-1);
+#undef TRACE_LAUNCH
+    CK(cudaGetLastError());
+    (*launches)++;
+    return FSLIC_OK;
+}
+
+// The cluster records after update `slot - 1`, i.e. after the prepare that finalised it (division, clamp, preemptive
+// bookkeeping; capi.cu splits the reference's update() across the assign kernel and that prepare).
+static int trace_clusters(fslic_ctx* c, const fslic_cluster* d_clusters, int batch, int slot, cudaStream_t st) {
+    const size_t rec = (size_t)c->K * sizeof(fslic_cluster);
+    CK(cudaMemcpy2DAsync(tr_clusters(c) + (size_t)slot * c->K, rec * c->tr_T, d_clusters, rec, rec, batch,
+                         cudaMemcpyDeviceToDevice, st));
+    return FSLIC_OK;
+}
+
 // Front half of iterate (context.cpp:114-181): Lab LUT, max_iter x (assign + update), full assign, for the
 // `batch` images starting at image `b0` of the context's buffers.  Leaves the pre-CCA labels in c->labels.
 static int iterate_front(fslic_ctx* c, int b0, const uint8_t* d_images, fslic_cluster* d_clusters, int batch,
@@ -1240,16 +1346,28 @@ static int iterate_front(fslic_ctx* c, int b0, const uint8_t* d_images, fslic_cl
         if (rc) return rc;
     }
     const fslic_cluster* cl = d_clusters;  // the NoQ variant reads its float centroids from the cluster records themselves
+    // debug_mode: snapshots between the stages below; a traced call never fuses the next prepare into an assign tail
+    const bool trace = c->trace_on;
+    if (trace) {
+        rc = trace_seed(c, d_clusters, batch, st, launches);
+        if (rc) return rc;
+    }
     int rem = 0;
     bool prepared = false;  // the previous assign+update launch already did the bookkeeping in its tail
     for (int it = 0; it < p->max_iter; it++) {
         if (!prepared) {
             rc = run_prepare(c, d_clusters, batch, it == 0, it > 0, st, launches, noq, preempt, 0);
             if (rc) return rc;
+            if (trace && it > 0) rc = trace_clusters(c, d_clusters, batch, it, st);
+            if (rc) return rc;
         }
         rc = run_assign_pass(c, batch, stride, rem, stride, it, true, coef, st, launches, variant, cl,
-                             variant < 0 ? d_clusters : nullptr, &prepared);
+                             variant < 0 && !trace ? d_clusters : nullptr, &prepared);
         if (rc) return rc;
+        if (trace) {
+            rc = trace_pass(c, batch, it, stride, rem, coef, variant, d_clusters, st, launches);
+            if (rc) return rc;
+        }
         if (variant == 4) {  // LSC: after_update (context.cpp:169-172); its Cluster update is the next prepare's
             rc = lsc_after_update(c, batch, stride, st, launches, timing);
             if (rc) return rc;
@@ -1258,8 +1376,18 @@ static int iterate_front(fslic_ctx* c, int b0, const uint8_t* d_images, fslic_cl
     }
     if (timing) CK(cudaEventRecord(c->ev[2], st));
     if (!prepared) {
-        rc = run_prepare(c, d_clusters, batch, p->max_iter == 0, p->max_iter > 0, st, launches, noq, preempt, 1);
+        // The last snapshot precedes PreemptiveGrid::finalize (context.cpp:173-176): a traced `preemptive` call lets this
+        // prepare derive the final update's active set like the earlier ones, records it, then sets every is_active.
+        const bool hold = trace && preempt && p->max_iter > 0;
+        rc = run_prepare(c, d_clusters, batch, p->max_iter == 0, p->max_iter > 0, st, launches, noq, preempt, hold ? 0 : 1);
         if (rc) return rc;
+        if (trace && p->max_iter > 0) rc = trace_clusters(c, d_clusters, batch, p->max_iter, st);
+        if (rc) return rc;
+        if (hold) {
+            k_trace_activate<<<ceil_div(batch * c->K, 256), 256, 0, st>>>(d_clusters, batch * c->K);
+            CK(cudaGetLastError());
+            (*launches)++;
+        }
     }
     rc = run_assign_pass(c, batch, 1, 0, stride, p->max_iter < stride ? p->max_iter : stride, false, coef, st, launches,
                          variant, cl);
@@ -1294,6 +1422,10 @@ static int iterate_plain(fslic_ctx* c, const uint8_t* d_images, fslic_cluster* d
     c->lev_used = 0;
     c->cca_timing = timing;
     c->cca_timed = false;
+    if (c->trace_on) {
+        rc = trace_begin(c, batch, p->max_iter, variant, st);
+        if (rc) return rc;
+    }
     if (timing) CK(cudaEventRecord(c->ev[0], st));
     rc = iterate_front(c, 0, d_images, d_clusters, batch, p, coef, st, &launches, timing, lab_done, variant);
     if (rc) return rc;
@@ -1350,7 +1482,8 @@ extern "C" int fslic_b200_cca_stage_ms(fslic_ctx* c, float* out_ms, int count) {
 // from then on.  Needs a capturable stream (not the legacy default stream) and no timing; anything else launches plainly.
 extern "C" int fslic_b200_iterate(fslic_ctx* c, const uint8_t* d_images, fslic_cluster* d_clusters, uint16_t* d_labels,
                                   int batch, const fslic_params* p, void* stream) {
-    if (c && p && c->graphs_enabled && batch > 0 && batch < 4 && p->collect_timing == 0 && stream != nullptr) {
+    // A traced call launches plainly and leaves the graph and its key alone: the next untraced call replays as before.
+    if (c && p && c->graphs_enabled && !c->trace_on && batch > 0 && batch < 4 && p->collect_timing == 0 && stream != nullptr) {
         fslic_ctx::GraphKey k;
         memset(&k, 0, sizeof(k));
         k.img = nullptr; k.cl = d_clusters; k.lab = d_labels; k.batch = batch; k.p = *p; k.manhattan = c->manhattan;
@@ -1529,6 +1662,7 @@ static int iterate_graphed(fslic_ctx* c, const uint8_t* d_images, fslic_cluster*
     // what the last plain build left), so after any graph launch the next plain call must rebuild them.
     if (c->gexec && memcmp(&k, &c->gkey, sizeof(k)) == 0) {
         CK(cudaGraphLaunch(c->gexec, st));
+        c->graph_replays++;
         c->spt_valid = false;
         c->last_launches = c->glaunches;
         c->disp = c->gdisp;
@@ -1559,6 +1693,7 @@ static int iterate_graphed(fslic_ctx* c, const uint8_t* d_images, fslic_cluster*
         return iterate_plain(c, d_images, d_clusters, d_labels, batch, p, st, true);
     }
     memcpy(&c->gkey, &k, sizeof(k));
+    c->graph_captures++;
     c->glaunches = c->last_launches;
     c->gdisp = c->disp;
     CK(cudaGraphLaunch(c->gexec, st));
@@ -1769,13 +1904,70 @@ static int iterate_host_enqueue(fslic_ctx* c, const uint8_t* h_images, fslic_clu
 
 extern "C" int fslic_b200_iterate_host(fslic_ctx* c, const uint8_t* h_images, fslic_cluster* h_clusters,
                                        uint16_t* h_labels, int batch, const fslic_params* p) {
+    if (c && c->trace_on) return set_err(FSLIC_EINVAL, "the host entry points are not traced: turn tracing off or use fslic_b200_iterate");
     return iterate_host_enqueue(c, h_images, h_clusters, h_labels, batch, p, true);
 }
 
 extern "C" int fslic_b200_iterate_host_async(fslic_ctx* c, const uint8_t* h_images, fslic_cluster* h_clusters,
                                              uint16_t* h_labels, int batch, const fslic_params* p) {
+    if (c && c->trace_on) return set_err(FSLIC_EINVAL, "the host entry points are not traced: turn tracing off or use fslic_b200_iterate");
     return iterate_host_enqueue(c, h_images, h_clusters, h_labels, batch, p, false);
 }
+
+// ---- debug_mode (trace.cuh, recorder_format.h) ---------------------------------------------------------------------
+extern "C" int fslic_b200_debug_graph_counts(const fslic_ctx* c, int* captures, int* replays) {
+    if (!c || !captures || !replays) return set_err(FSLIC_EINVAL, "NULL argument");
+    *captures = c->graph_captures;
+    *replays = c->graph_replays;
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_set_trace(fslic_ctx* c, int on) {
+    if (!c || c->cca_only) return set_err(FSLIC_EINVAL, "NULL or connectivity-only context");
+    c->trace_on = on != 0;
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_trace_info(const fslic_ctx* c, int* snapshots, int* batch, int* dist_bytes) {
+    if (!c || !snapshots || !batch || !dist_bytes) return set_err(FSLIC_EINVAL, "NULL argument");
+    *snapshots = c->tr_T;
+    *batch = c->tr_B;
+    *dist_bytes = c->tr_dist_bytes;
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_trace_snapshots(fslic_ctx* c, int image, uint16_t* h_assignment, void* h_min_dists,
+                                          fslic_cluster* h_clusters, uint32_t* h_mismatches) {
+    if (!c) return set_err(FSLIC_EINVAL, "NULL context");
+    if (c->tr_T == 0) return set_err(FSLIC_EINVAL, "no traced iterate has been recorded on this context");
+    if (image < 0 || image >= c->tr_B) return set_err(FSLIC_EINVAL, "image outside the traced batch");
+    USE_DEVICE(c->device);
+    CK(cudaDeviceSynchronize());
+    const size_t T = c->tr_T, N = c->N, K = c->K, slot = (size_t)image * T;
+    if (h_clusters) CK(cudaMemcpy(h_clusters, tr_clusters(c) + slot * K, T * K * sizeof(fslic_cluster), cudaMemcpyDeviceToHost));
+    if (h_min_dists)
+        CK(cudaMemcpy(h_min_dists, tr_dist(c) + slot * N * c->tr_dist_bytes, T * N * c->tr_dist_bytes, cudaMemcpyDeviceToHost));
+    if (h_assignment) CK(cudaMemcpy(h_assignment, tr_assign(c) + slot * N, T * N * 2, cudaMemcpyDeviceToHost));
+    uint32_t bad = 0;
+    CK(cudaMemcpy(&bad, c->tr_bad, sizeof(bad), cudaMemcpyDeviceToHost));
+    if (h_mismatches) *h_mismatches = bad;
+    if (bad)
+        return set_err(FSLIC_ECHECK, "debug_mode self-check: " + std::to_string(bad) +
+                                         " pixels were labelled differently from the trace kernel's argmin");
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_format_report(int H, int W, int K, int snapshots, int dist_is_float, const uint16_t* assignment,
+                                        const void* min_dists, const fslic_cluster* clusters, char** out, size_t* len) {
+    if (!out || !len || H < 0 || W < 0 || K < 0 || snapshots < 0) return set_err(FSLIC_EINVAL, "bad argument");
+    if (snapshots > 0 && ((H * W > 0 && (!assignment || !min_dists)) || (K > 0 && !clusters)))
+        return set_err(FSLIC_EINVAL, "NULL array");
+    *out = recorder_fmt::format_report(H, W, K, snapshots, dist_is_float != 0, assignment, min_dists, clusters, len);
+    if (!*out) return set_err(FSLIC_ENOMEM, "out of host memory (debug_mode report)");
+    return FSLIC_OK;
+}
+
+extern "C" void fslic_b200_free_report(char* p) { free(p); }
 
 extern "C" int fslic_b200_wait(fslic_ctx* c) {
     if (!c) return set_err(FSLIC_EINVAL, "ctx is NULL");

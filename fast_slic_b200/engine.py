@@ -278,3 +278,39 @@ class Engine:
 
     def launches_last_iterate(self):
         return int(self._L.fslic_b200_launches_last_iterate(self._h))
+
+    def graph_counts(self):
+        """(captures, replays): CUDA graphs iterate() captured and replays it launched on this context so far."""
+        cap, rep = C.c_int(), C.c_int()
+        check(self._L.fslic_b200_debug_graph_counts(self._h, C.byref(cap), C.byref(rep)))
+        return int(cap.value), int(rep.value)
+
+    # -- debug_mode (fslic_b200_set_trace) ----------------------------------------------------------
+    def set_trace(self, on):
+        """With tracing on, iterate / iterate_real / iterate_preemptive / iterate_lsc record the reference's debug_mode snapshots of
+        every image (same labels and clusters as untraced); the host entry points refuse to run."""
+        with self.lock:
+            check(self._L.fslic_b200_set_trace(self._h, int(bool(on))))
+
+    def trace_snapshots(self, image=0):
+        """Snapshots of image `image` of the last traced call (synchronises the device):
+        {"iterations": int32[T] (-1, 0, ..), "assignment": u16[T, H, W], "min_dists": u16 or float32 [T, H, W],
+        "clusters": CLUSTER_DTYPE[T, K], "mismatches": int}.  Raises FslicError when an assign kernel disagreed with the
+        trace kernel on any pixel."""
+        T, B, db = C.c_int(), C.c_int(), C.c_int()
+        check(self._L.fslic_b200_trace_info(self._h, C.byref(T), C.byref(B), C.byref(db)))
+        T = T.value
+        assign = np.empty((T, self.H, self.W), np.uint16)
+        dist = np.empty((T, self.H, self.W), np.float32 if db.value == 4 else np.uint16)
+        clusters = np.empty((T, self.K), CLUSTER_DTYPE)
+        bad = C.c_uint32()
+        with self.lock:
+            check(self._L.fslic_b200_trace_snapshots(self._h, int(image), assign.ctypes.data, dist.ctypes.data,
+                                                     clusters.ctypes.data, C.byref(bad)))
+        return {"iterations": np.arange(-1, T - 1, dtype=np.int32), "assignment": assign, "min_dists": dist,
+                "clusters": clusters, "mismatches": int(bad.value)}
+
+    def recorder_report(self, image=0):
+        """The reference's last_recorder_report bytes for image `image` of the last traced call."""
+        s = self.trace_snapshots(image)
+        return _lib.format_recorder_report(self.H, self.W, s["assignment"], s["min_dists"], s["clusters"])

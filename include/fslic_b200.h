@@ -52,7 +52,8 @@ enum {
     FSLIC_ECUDA = -2,    /* CUDA runtime error */
     FSLIC_ENOMEM = -3,
     FSLIC_ERANGE = -4,   /* compactness so large the u16 distance would overflow (UB in the reference) */
-    FSLIC_ENOFRAME = -5  /* CRF: no frame with that time (reference: std::out_of_range, IndexError in Python) */
+    FSLIC_ENOFRAME = -5, /* CRF: no frame with that time (reference: std::out_of_range, IndexError in Python) */
+    FSLIC_ECHECK = -6    /* debug_mode: an assign pass disagreed with the trace kernel (fslic_b200_trace_snapshots) */
 };
 
 typedef struct fslic_ctx fslic_ctx;
@@ -147,6 +148,33 @@ int fslic_b200_initialize_clusters_host(fslic_ctx* ctx, const uint8_t* h_images,
 int fslic_b200_iterate_host_async(fslic_ctx* ctx, const uint8_t* h_images, fslic_cluster* h_clusters,
                                   uint16_t* h_labels, int batch, const fslic_params* params);
 int fslic_b200_wait(fslic_ctx* ctx);
+
+/* == debug_mode (context.h:36; the Recorder of recorder.h, pushed at context.cpp:157,173).  With tracing on, every
+ *    image of a fslic_b200_iterate, fslic_b200_iterate_real, fslic_b200_iterate_preemptive or fslic_b200_iterate_lsc
+ *    call records T = max_iter + 1 snapshots: s = 0 after seeding (the reference's iteration -1), s = i + 1 after
+ *    update i.  Each holds the pre-CCA assignment u16[H*W], the per-pixel minimum distance min_dists[H*W] (u16 for the
+ *    default contexts and `preemptive`, float for the float-distance ones and LSC) and the K cluster records.  Labels
+ *    and clusters are those of the untraced call; a traced call takes plain launches (no graph replay, no fused
+ *    prepare) and a trace kernel per pass that also checks the pass's labels.  Snapshots go to device buffers grown on
+ *    demand (T * B * (H*W*(2 + 2 or 4) + K*32) bytes; FSLIC_ENOMEM when they cannot be had).  While tracing is on the
+ *    host entry points return FSLIC_EINVAL. */
+int fslic_b200_set_trace(fslic_ctx* ctx, int on);
+/* CUDA graphs fslic_b200_iterate captured and replays it launched on this context so far (diagnostics). */
+int fslic_b200_debug_graph_counts(const fslic_ctx* ctx, int* captures, int* replays);
+/* What the last traced call recorded: snapshots T (0: none), batch B, bytes per min_dists entry (2 or 4). */
+int fslic_b200_trace_info(const fslic_ctx* ctx, int* snapshots, int* batch, int* dist_bytes);
+/* Synchronises the device and copies image `image`'s snapshots to host arrays (any may be NULL): h_assignment
+ * u16[T][H*W], h_min_dists [T][H*W] of the recorded type, h_clusters [T][K].  *h_mismatches gets the number of pixels
+ * whose label an assign kernel set differently from the trace kernel's argmin over the whole traced call; a nonzero
+ * count also returns FSLIC_ECHECK. */
+int fslic_b200_trace_snapshots(fslic_ctx* ctx, int image, uint16_t* h_assignment, void* h_min_dists,
+                               fslic_cluster* h_clusters, uint32_t* h_mismatches);
+/* Host only (no CUDA call): the text of Recorder::get_report (recorder.h:18-47, 90-98) for `snapshots` snapshots laid
+ * out like fslic_b200_trace_snapshots' arrays (iterations -1, 0, 1, ...; min_dists float when dist_is_float, else u16).
+ * *out gets a malloc'd NUL-terminated buffer of *len bytes, to be released with fslic_b200_free_report. */
+int fslic_b200_format_report(int H, int W, int K, int snapshots, int dist_is_float, const uint16_t* assignment,
+                             const void* min_dists, const fslic_cluster* clusters, char** out, size_t* len);
+void fslic_b200_free_report(char* report);
 
 /* == cca::ConnectivityEnforcer(labels,H,W,K,min_threshold).execute(labels) (cca.cpp:178-265),
  *    in place on d_labels [B,H,W] u16.  H, W come from the context; K (= max label + 1 in
