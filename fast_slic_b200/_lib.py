@@ -30,6 +30,8 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_crf_temporal_pairwise_energy", "fslic_b200_debug_expf_host", "fslic_b200_debug_expf_device",
     "fslic_b200_set_trace", "fslic_b200_trace_info", "fslic_b200_trace_snapshots", "fslic_b200_format_report",
     "fslic_b200_free_report", "fslic_b200_debug_graph_counts",
+    "fslic_b200_connectivity_batch_scratch_bytes", "fslic_b200_get_connectivity_batch",
+    "fslic_b200_get_mask_density_batch", "fslic_b200_cluster_density_to_mask_batch",
 )
 
 STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity", "iterate")
@@ -103,6 +105,11 @@ def lib():
     L.fslic_b200_get_connectivity.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, C.c_size_t, vp]
     L.fslic_b200_get_mask_density.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
     L.fslic_b200_cluster_density_to_mask.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp]
+    L.fslic_b200_connectivity_batch_scratch_bytes.argtypes = [i32, i32]
+    L.fslic_b200_connectivity_batch_scratch_bytes.restype = C.c_size_t
+    L.fslic_b200_get_connectivity_batch.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, C.c_size_t, vp]
+    L.fslic_b200_get_mask_density_batch.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
+    L.fslic_b200_cluster_density_to_mask_batch.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp]
     L.fslic_b200_assign_kernel_time.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]
     L.fslic_b200_debug_cca_counters.argtypes = [vp, C.POINTER(C.c_int32), i32]
     L.fslic_b200_debug_select_profile.argtypes = [vp, C.POINTER(C.c_longlong), i32]

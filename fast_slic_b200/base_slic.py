@@ -13,7 +13,7 @@ import threading
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, graph_batch
 from .engine import CLUSTER_DTYPE, Engine, require_cuda
 
 ARCH_NAME = "cuda/sm_90a"
@@ -506,6 +506,24 @@ class BaseSlic(object):
                     clusters = eng.initialize_clusters_host(images)
                 labels = eng.iterate_host(images, clusters, params, **spatial)
         return (labels, clusters) if return_clusters else labels
+
+    def get_connectivity_batch(self, labels, return_replayed=False):
+        """int16 labels [B,H,W] (numpy or cuda tensor) -> (counts int32[B,K], neighbors int32[B,K,12]) of the same kind:
+        image b's graph is `NodeConnectivity(counts[b], neighbors[b])`, equal to `slic_model.get_connectivity(labels[b])`
+        (entries past a count are 0).  With `return_replayed`, also int32[B]: 1 for an image with so many distinct
+        adjacent label pairs that it took the exact single-thread replay of the reference's scan."""
+        return graph_batch.get_connectivity_batch(self.num_components, self._slic_model.device, labels, return_replayed)
+
+    def get_mask_density_batch(self, masks, labels, clusters):
+        """uint8 masks [B,H,W] and int16 labels [B,H,W] with the clusters `iterate_batch` returned ([B,K] structured
+        array / [B,K,32] uint8 cuda tensor) -> uint8[B,K], image b equal to `slic_model.get_mask_density`."""
+        return graph_batch.get_mask_density_batch(self.num_components, self._slic_model.device, masks, labels, clusters)
+
+    def broadcast_density_to_mask_batch(self, densities, labels):
+        """uint8 densities [B,K] and int16 labels [B,H,W] -> uint8[B,H,W], image b equal to
+        `slic_model.broadcast_density_to_mask`."""
+        return graph_batch.broadcast_density_to_mask_batch(self.num_components, self._slic_model.device, densities,
+                                                           labels)
 
 
 class Slic(BaseSlic):

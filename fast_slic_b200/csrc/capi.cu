@@ -3,6 +3,7 @@
 // Plays the role of BaseContext<uint16_t>::iterate (fast-slic/src/context.cpp:109-197) and of
 // the Cython glue that drives it (cfast_slic.pyx:124-197): owns the scratch buffers, sequences the
 // kernels on one stream, never touches the CPU for the data path.
+#include <limits.h>
 #include <math.h>
 #include <stdlib.h>
 #include <new>
@@ -16,6 +17,7 @@
 #include "assign.cuh"
 #include "assign5.cuh"
 #include "graph.cuh"
+#include "graph_batch.cuh"
 #include "realdist.cuh"
 #include "lsc.cuh"
 #include "crf.cuh"
@@ -2075,6 +2077,105 @@ extern "C" int fslic_b200_cluster_density_to_mask(int device, int H, int W, int 
     const long cap = grid_stride_cap(device);
     if (blocks > cap) blocks = cap;
     k_density_broadcast<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(d_labels, d_densities, n, K, d_result);
+    CK(cudaGetLastError());
+    return FSLIC_OK;
+}
+
+// ---- the same consumers over a batch of label maps (graph_batch.cuh): stateless, asynchronous, never synchronise ----
+static int bit_length(unsigned long long v) {
+    int n = 0;
+    for (; v; v >>= 1) n++;
+    return n;
+}
+static size_t connb_sort_temp_bytes(long long items, int end_bit) {
+    size_t bytes = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                    (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)items, 0, end_bit);
+    return bytes;
+}
+static long grid_for(long items, int device) {
+    long blocks = (items + 255) / 256;
+    const long cap = grid_stride_cap(device);
+    return blocks < 1 ? 1 : (blocks > cap ? cap : blocks);
+}
+
+// Key and order tables, their sorted copies, the sort's temporary storage (sized for all 64 key bits, an upper bound
+// of what a call sorts) and the per-image overflow flags.
+extern "C" size_t fslic_b200_connectivity_batch_scratch_bytes(int K, int batch) {
+    if (K <= 0 || batch <= 0) return 256;
+    if (K > 65535) return (size_t)-1;
+    const long long slots = (long long)conn_table_size(K) * batch;
+    if (slots > INT_MAX) return (size_t)-1;  // more than one radix sort takes: the call refuses such a batch
+    return align_up((size_t)slots * 4, 256) * 2 + align_up((size_t)slots * 8, 256) * 2 +
+           align_up(connb_sort_temp_bytes(slots, 64), 256) + align_up((size_t)batch * 4, 256);
+}
+
+extern "C" int fslic_b200_get_connectivity_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels,
+                                                 int32_t* d_counts, uint32_t* d_neighbors, int32_t* d_replayed,
+                                                 void* d_scratch, size_t scratch_bytes, void* stream) {
+    if (batch < 0 || H <= 0 || W <= 0 || K <= 0 || K > 65535) return set_err(FSLIC_EINVAL, "bad batch, H, W or K");
+    if (batch == 0) return FSLIC_OK;
+    if (!d_labels || !d_counts || !d_neighbors || !d_scratch) return set_err(FSLIC_EINVAL, "NULL argument");
+    const uint32_t T = conn_table_size(K);
+    const long long slots = (long long)T * batch;
+    if (slots > INT_MAX) return set_err(FSLIC_EINVAL, "batch too large for one call: the pair tables exceed 2^31 slots");
+    const int obits = bit_length(3ull * (unsigned long long)H * (unsigned long long)W), bits = obits + bit_length(batch - 1);
+    if (bits > 64) return set_err(FSLIC_EINVAL, "batch * H * W too large");
+    USE_DEVICE(device);
+    if (scratch_bytes < fslic_b200_connectivity_batch_scratch_bytes(K, batch)) return set_err(FSLIC_EINVAL, "scratch too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    unsigned char* p = static_cast<unsigned char*>(d_scratch);
+    uint32_t* tkey = reinterpret_cast<uint32_t*>(p); p += align_up((size_t)slots * 4, 256);
+    uint32_t* skey = reinterpret_cast<uint32_t*>(p); p += align_up((size_t)slots * 4, 256);
+    unsigned long long* tord = reinterpret_cast<unsigned long long*>(p); p += align_up((size_t)slots * 8, 256);
+    unsigned long long* sord = reinterpret_cast<unsigned long long*>(p); p += align_up((size_t)slots * 8, 256);
+    size_t temp_bytes = align_up(connb_sort_temp_bytes(slots, 64), 256);
+    if (connb_sort_temp_bytes(slots, bits) > temp_bytes) return set_err(FSLIC_ECUDA, "radix sort temporary storage");
+    void* temp = p; p += temp_bytes;
+    int* overflow = reinterpret_cast<int*>(p);
+    // the walk's shared memory: u8 counts of the K labels + the staged chunk; opted in once per device for any K
+    const int smem = ((K + 15) & ~15) + CONNB_CHUNK * 4, smem_max = 65536 + CONNB_CHUNK * 4;
+    static bool walk_smem_set[64] = {};
+    if (device < 0 || device >= 64 || !walk_smem_set[device]) {
+        CK(cudaFuncSetAttribute(k_connb_walk, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+        if (device >= 0 && device < 64) walk_smem_set[device] = true;
+    }
+    k_connb_init<<<(int)grid_for(slots, device), 256, 0, st>>>(tkey, tord, slots, bit_length(T) - 1, obits, batch, overflow);
+    const long n = (long)batch * (H - 1) * (W - 1);
+    if (n > 0)
+        k_connb_discover<<<(int)grid_for(n, device), 256, 0, st>>>(d_labels, batch, H, W, K, tkey, tord, T, obits, overflow);
+    if (cub::DeviceRadixSort::SortPairs(temp, temp_bytes, tord, sord, tkey, skey, (int)slots, 0, bits, st) != cudaSuccess)
+        return set_err(FSLIC_ECUDA, "radix sort of the pair tables failed");
+    k_connb_walk<<<batch, 256, smem, st>>>(skey, T, d_labels, H, W, K, overflow, d_counts, d_neighbors, d_replayed);
+    CK(cudaGetLastError());
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_get_mask_density_batch(int device, int batch, int H, int W, int K, const fslic_cluster* d_clusters,
+                                                 const uint16_t* d_labels, const uint8_t* d_masks, uint8_t* d_densities,
+                                                 int32_t* d_scratch, void* stream) {
+    if (batch < 0 || H <= 0 || W <= 0 || K <= 0 || K > 65535) return set_err(FSLIC_EINVAL, "bad batch, H, W or K");
+    if (batch == 0) return FSLIC_OK;
+    if (!d_clusters || !d_labels || !d_masks || !d_densities || !d_scratch) return set_err(FSLIC_EINVAL, "NULL argument");
+    USE_DEVICE(device);
+    cudaStream_t st = (cudaStream_t)stream;
+    const long n = (long)H * W, nk = (long)batch * K;
+    CK(cudaMemsetAsync(d_scratch, 0, (size_t)nk * 4, st));
+    k_mask_sum_batch<<<(int)grid_for(n * batch, device), 256, 0, st>>>(d_labels, d_masks, n, batch, K, d_scratch);
+    k_density_final_batch<<<(int)grid_for(nk, device), 256, 0, st>>>(d_scratch, d_clusters, nk, d_densities);
+    CK(cudaGetLastError());
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_cluster_density_to_mask_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels,
+                                                        const uint8_t* d_densities, uint8_t* d_result, void* stream) {
+    if (batch < 0 || H <= 0 || W <= 0 || K <= 0 || K > 65535) return set_err(FSLIC_EINVAL, "bad batch, H, W or K");
+    if (batch == 0) return FSLIC_OK;
+    if (!d_labels || !d_densities || !d_result) return set_err(FSLIC_EINVAL, "NULL argument");
+    USE_DEVICE(device);
+    const long n = (long)H * W;
+    k_density_broadcast_batch<<<(int)grid_for(n * batch, device), 256, 0, (cudaStream_t)stream>>>(d_labels, d_densities, n,
+                                                                                                   batch, K, d_result);
     CK(cudaGetLastError());
     return FSLIC_OK;
 }

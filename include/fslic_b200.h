@@ -197,6 +197,27 @@ int fslic_b200_get_mask_density(int device, int H, int W, int K, const fslic_clu
 int fslic_b200_cluster_density_to_mask(int device, int H, int W, int K, const uint16_t* d_labels, const uint8_t* d_densities,
                                        uint8_t* d_result, void* stream);
 
+/* The three consumers above over `batch` label maps d_labels u16[B,H,W], each image on its own: every image's result is
+ * what the single-image call gives for it.  Asynchronous on `stream` and never synchronise, so a CUDA graph can capture
+ * them; batch == 0 does nothing.
+ * Connectivity: d_counts int32[B,K], d_neighbors u32[B,K,12] (zero past the count); d_replayed int32[B] (or NULL)
+ * receives 1 for an image whose pair table overflowed and took the exact single-thread replay of the reference's loop,
+ * else 0.  d_scratch holds fslic_b200_connectivity_batch_scratch_bytes(K, batch) bytes: 24 * B * T for the pair tables
+ * (T = the table size of fslic_b200_connectivity_scratch_bytes, a power of two >= max(4096, 32 * K)), plus the radix
+ * sort's temporary storage for B * T pairs, plus 4 * B; 256 for K <= 0 or B <= 0; (size_t)-1 for K > 65535 or when
+ * B * T exceeds 2^31 - 1 (split the batch). */
+size_t fslic_b200_connectivity_batch_scratch_bytes(int K, int batch);
+int fslic_b200_get_connectivity_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels,
+                                      int32_t* d_counts, uint32_t* d_neighbors, int32_t* d_replayed, void* d_scratch,
+                                      size_t scratch_bytes, void* stream);
+/* d_clusters [B,K], d_masks u8[B,H,W], d_densities u8[B,K]; d_scratch int32[B,K]. */
+int fslic_b200_get_mask_density_batch(int device, int batch, int H, int W, int K, const fslic_cluster* d_clusters,
+                                      const uint16_t* d_labels, const uint8_t* d_masks, uint8_t* d_densities,
+                                      int32_t* d_scratch, void* stream);
+/* d_densities u8[B,K] -> d_result u8[B,H,W] (0 where the label is >= K). */
+int fslic_b200_cluster_density_to_mask_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels,
+                                             const uint8_t* d_densities, uint8_t* d_result, void* stream);
+
 /* Stage probes for the parity tests (the reference's protected quad_image / assignment,
  * context.h:48-50): copies of the last iterate()'s Lab quad image [B,H,W,4] u8 and pre-CCA
  * labels [B,H,W] u16 into caller device buffers (either may be NULL). */
