@@ -32,6 +32,9 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_free_report", "fslic_b200_debug_graph_counts",
     "fslic_b200_connectivity_batch_scratch_bytes", "fslic_b200_get_connectivity_batch",
     "fslic_b200_get_mask_density_batch", "fslic_b200_cluster_density_to_mask_batch",
+    "fslic_b200_crfdev_push_scratch_bytes", "fslic_b200_crfdev_push_label_frames", "fslic_b200_crfdev_set_unary",
+    "fslic_b200_crfdev_set_proba", "fslic_b200_crfdev_set_mask", "fslic_b200_crfdev_get_inferred",
+    "fslic_b200_debug_logf_host", "fslic_b200_debug_logf_device",
 )
 
 STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity", "iterate")

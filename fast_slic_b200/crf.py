@@ -10,7 +10,22 @@ Typical use is temporal smoothing of per-superpixel class probabilities across v
     q = frame.get_inferred()
 
 Unary setters take host arrays, like the reference's memoryviews; `inference` runs asynchronously on the device and
-the getters wait for it.  Where the reference reads out of bounds or crashes, this module raises instead: neighbour
+the getters wait for it.
+
+The CRF can also be fed from the device, with no host round trip: `SimpleCRF.push_label_frames` takes the int16 cuda
+labels and uint8 [K,32] cluster records that `iterate_batch(..., return_clusters=True)` returns, and `set_proba`,
+`set_mask`, the `unaries` setter and `get_inferred(out=...)` take cuda tensors::
+
+    labels, clusters = slic.iterate_batch(images, return_clusters=True)    # cuda tensors [B,H,W], [B,K,32]
+    frames = crf.push_label_frames(labels, clusters)                       # B frames
+    frames[-1].set_proba(proba)                                            # float32 cuda [C, K]
+    crf.initialize(); crf.inference(5)
+    frames[-1].get_inferred(out=q)                                         # float32 cuda [C, K]
+
+That work is enqueued on the CRF device's current torch stream, and every frame equals what the host path stores for
+the same values, bit for bit.
+
+Where the reference reads out of bounds or crashes, this module raises instead: neighbour
 indices or mask classes outside the frame raise ValueError and change nothing, and a frame handle whose frame was
 popped raises IndexError.
 """
@@ -19,6 +34,7 @@ import operator
 import threading
 
 import numpy as np
+import torch
 
 from . import _lib
 from .engine import CLUSTER_DTYPE
@@ -63,6 +79,14 @@ def _L():
         L.fslic_b200_crf_temporal_pairwise_energy.argtypes = [vp, i32, i32, vp, i32, C.POINTER(C.c_float)]
         L.fslic_b200_debug_expf_host.argtypes = [C.c_uint32, ll, vp]
         L.fslic_b200_debug_expf_device.argtypes = [i32, C.c_uint32, ll, vp, vp]
+        L.fslic_b200_debug_logf_host.argtypes = [C.c_uint32, ll, vp]
+        L.fslic_b200_debug_logf_device.argtypes = [i32, C.c_uint32, ll, vp, vp]
+        L.fslic_b200_crfdev_push_scratch_bytes.argtypes = [i32, i32]
+        L.fslic_b200_crfdev_push_scratch_bytes.restype = C.c_size_t
+        L.fslic_b200_crfdev_push_label_frames.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, C.c_size_t, vp, ip]
+        for name in ("set_unary", "set_proba", "get_inferred"):
+            getattr(L, "fslic_b200_crfdev_" + name).argtypes = [vp, i32, vp, vp]
+        L.fslic_b200_crfdev_set_mask.argtypes = [vp, i32, vp, C.c_float, vp]
         _bound = True
     return L
 
@@ -114,6 +138,23 @@ def _vp(a):
     return a.ctypes.data_as(C.c_void_p)
 
 
+def _is_cuda(x):
+    """A cuda tensor takes the device path; anything else the host path, unchanged."""
+    return isinstance(x, torch.Tensor) and x.is_cuda
+
+
+def _device_tensor(x, device, dtype, ndim, cname):
+    """A cuda tensor argument of the device path: `dtype`, rank `ndim`, on cuda:`device`; ValueError otherwise, like
+    `_buffer`'s errors."""
+    if x.dtype != dtype:
+        raise ValueError("Buffer dtype mismatch, expected '%s' but got '%s'" % (cname, x.dtype))
+    if x.dim() != ndim:
+        raise ValueError("Buffer has wrong number of dimensions (expected %d, got %d)" % (ndim, x.dim()))
+    if x.device != torch.device("cuda", device):
+        raise ValueError("tensor is on %s, the CRF on cuda:%d" % (x.device, device))
+    return x
+
+
 class SimpleCRFFrame(object):
     """== csimple_crf.SimpleCRFFrame: a handle on one frame of `parent_crf` (which it keeps alive)."""
 
@@ -152,6 +193,12 @@ class SimpleCRFFrame(object):
         with p.lock:
             _check(getattr(_L(), "fslic_b200_crf_" + name)(p._h, self._time, *args))
 
+    def _dcall(self, name, *args):
+        """A device-feed entry point, on the CRF device's current torch stream."""
+        p = self._parent
+        with p.lock:
+            _check(getattr(_L(), "fslic_b200_crfdev_" + name)(p._h, self._time, *args, p._stream()))
+
     def _fresh_buffer(self):
         return np.zeros([self.num_classes, self.num_nodes], dtype=np.float32)
 
@@ -163,6 +210,10 @@ class SimpleCRFFrame(object):
 
     @unaries.setter
     def unaries(self, new_value):
+        if _is_cuda(new_value):
+            a = self._check_dimension(_device_tensor(new_value, self._parent.device, torch.float32, 2, "float"))
+            self._dcall("set_unary", a.contiguous().data_ptr())
+            return
         a = self._check_dimension(_buffer(new_value, np.float32, 2, "float"))
         self._call("set_unary", _vp(a))
 
@@ -228,6 +279,14 @@ class SimpleCRFFrame(object):
         self._call("set_unbiased")
 
     def set_mask(self, classes, confidence):
+        if _is_cuda(classes):  # classes are checked on the device: out of range raises ValueError, nothing changes
+            a = _device_tensor(classes, self._parent.device, torch.int32, 1, "int")
+            confidence = float(confidence)
+            if a.shape[0] != self.num_nodes:
+                raise ValueError("The dimension of class array should match the number of nodes {}".format(
+                    self.num_nodes))
+            self._dcall("set_mask", a.contiguous().data_ptr(), C.c_float(confidence))
+            return
         a = _buffer(classes, np.int32, 1, "int")
         confidence = float(confidence)
         if a.shape[0] != self.num_nodes:
@@ -237,10 +296,24 @@ class SimpleCRFFrame(object):
         self._call("set_mask", _vp(a), C.c_float(confidence))
 
     def set_proba(self, proba):
+        if _is_cuda(proba):
+            a = self._check_dimension(_device_tensor(proba, self._parent.device, torch.float32, 2, "float"))
+            self._dcall("set_proba", a.contiguous().data_ptr())
+            return
         a = self._check_dimension(_buffer(proba, np.float32, 2, "float"))
         self._call("set_proba", _vp(a))
 
-    def get_inferred(self):
+    def get_inferred(self, out=None):
+        """q as a new float32 [C, N] numpy array; or, given a contiguous cuda float32 [C, N] tensor `out`, q copied into
+        it on the current stream, and `out` returned."""
+        if out is not None:
+            if not _is_cuda(out):
+                raise ValueError("out must be a cuda float32 tensor of shape [num_classes, num_nodes]")
+            self._check_dimension(_device_tensor(out, self._parent.device, torch.float32, 2, "float"))
+            if not out.is_contiguous():
+                raise ValueError("out must be contiguous")
+            self._dcall("get_inferred", out.data_ptr())
+            return out
         out = self._fresh_buffer()
         self._call("get_inferred", _vp(out))
         return out
@@ -367,6 +440,50 @@ class SimpleCRF(object):
         frame.set_connectivity(conn)
         frame.set_unbiased()
         return frame
+
+    def push_label_frames(self, labels, clusters):
+        """Frames from device tensors: int16 cuda labels [H,W] or [B,H,W] and the uint8 [K,32] / [B,K,32] cluster
+        records of the same images, as `iterate_batch(..., return_clusters=True)` returns them.  Frame b equals what
+        push_slic_frame gives for a Slic whose last_assignment is labels[b] and whose records are clusters[b]: the
+        records truncated to int32 as there, the adjacency graph of labels[b] (labels outside [0, K) ignored) and
+        unbiased unaries.  Returns one SimpleCRFFrame for [H,W] labels, a list for [B,H,W].  Enqueued on the CRF
+        device's current torch stream.  Unlike push_slic_frame, which pushes a blank frame before it fails on
+        K != num_nodes, this checks every argument (ValueError) before anything is pushed."""
+        from .graph_batch import graph_chunk
+        if not _is_cuda(labels) or not _is_cuda(clusters):
+            raise ValueError("labels and clusters must be cuda tensors (push_slic_frame takes host arrays)")
+        single = labels.dim() == 2
+        _device_tensor(labels, self.device, torch.int16, 2 if single else 3, "int16_t")
+        _device_tensor(clusters, self.device, torch.uint8, 2 if single else 3, "uint8_t")
+        lab = labels[None] if single else labels
+        cl = clusters[None] if single else clusters
+        B, H, W = (int(v) for v in lab.shape)
+        if tuple(cl.shape) != (B, self._N, 32):
+            raise ValueError("clusters must be %s with K = num_nodes, got %s" % (
+                (self._N, 32) if single else (B, self._N, 32), tuple(clusters.shape)))
+        if H == 0 or W == 0:
+            raise ValueError("labels must have at least one pixel")
+        if not 1 <= self._N <= 65535:
+            raise ValueError("push_label_frames needs 1 <= num_nodes <= 65535, the range of the labels")
+        lab, cl = lab.contiguous(), cl.contiguous()
+        times = np.zeros(B, np.int32)
+        if B:
+            L = _L()
+            dev = torch.device("cuda", self.device)
+            with torch.cuda.device(dev), self.lock:
+                chunk = graph_chunk(self._N, B)  # images whose graph scratch stays under GRAPH_SCRATCH_CAP
+                nbytes = int(L.fslic_b200_crfdev_push_scratch_bytes(self._N, chunk))
+                scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+                for b0 in range(0, B, chunk):
+                    n = min(chunk, B - b0)
+                    _check(L.fslic_b200_crfdev_push_label_frames(
+                        self._h, n, H, W, self._N, lab[b0].data_ptr(), cl[b0].data_ptr(), scratch.data_ptr(), nbytes,
+                        self._stream(), times[b0:].ctypes.data_as(C.POINTER(C.c_int))))
+        frames = [SimpleCRFFrame(self, int(t)) for t in times]
+        return frames[0] if single else frames
+
+    def _stream(self):
+        return C.c_void_p(torch.cuda.current_stream(torch.device("cuda", self.device)).cuda_stream)
 
     def push_frame(self):
         t = C.c_int()

@@ -21,6 +21,7 @@
 #include "realdist.cuh"
 #include "lsc.cuh"
 #include "crf.cuh"
+#include "crf_feed.cuh"
 #include "preempt.cuh"
 #include "cca.cuh"
 #include "common.cuh"
@@ -2198,6 +2199,7 @@ struct CrfSlot {
     float *unary = nullptr, *q0 = nullptr, *q1 = nullptr, *msg = nullptr, *tmp = nullptr;
     std::vector<fslic_cluster> h_clusters;
     std::vector<int32_t> h_off, h_nbr;
+    bool h_stale = false;  // a device push (fslic_b200_crfdev_push_label_frames) wrote the frame: h_* are out of date
 };
 
 struct fslic_crf {
@@ -2351,6 +2353,7 @@ extern "C" int fslic_b200_crf_push_frame(fslic_crf* c, int* time_out) {
     s->h_clusters.assign(N, blank);
     s->h_off.assign(N + 1, 0);
     s->h_nbr.clear();
+    s->h_stale = false;
     if (N) CK(cudaMemcpyAsync(s->clusters, s->h_clusters.data(), sizeof(fslic_cluster) * N, cudaMemcpyHostToDevice, c->st));
     CK(cudaMemsetAsync(s->offsets, 0, sizeof(int32_t) * (N + 1), c->st));
     if (CN) {
@@ -2387,6 +2390,27 @@ extern "C" int fslic_b200_crf_pop_frame(fslic_crf* c, int* time_out) {
     return crf_upload_table(c);
 }
 
+// Brings the host copies of a device-pushed frame up to date: one wait for the CRF's stream and a download of its
+// records and CSR.  Every reader of h_clusters / h_off / h_nbr calls it first; for a host-fed frame it does nothing.
+static int crf_refresh_host(fslic_crf* c, CrfSlot* s) {
+    if (!s->h_stale) return FSLIC_OK;
+    USE_DEVICE(c->device);
+    const int N = c->N;
+    s->h_clusters.resize(N);
+    s->h_off.resize(N + 1);
+    CK(cudaStreamSynchronize(c->st));
+    if (N) CK(cudaMemcpyAsync(s->h_clusters.data(), s->clusters, sizeof(fslic_cluster) * N, cudaMemcpyDeviceToHost, c->st));
+    CK(cudaMemcpyAsync(s->h_off.data(), s->offsets, sizeof(int32_t) * (N + 1), cudaMemcpyDeviceToHost, c->st));
+    CK(cudaStreamSynchronize(c->st));
+    s->h_nbr.resize(s->h_off[N]);
+    if (s->h_off[N]) {
+        CK(cudaMemcpyAsync(s->h_nbr.data(), s->nbr, sizeof(int32_t) * s->h_off[N], cudaMemcpyDeviceToHost, c->st));
+        CK(cudaStreamSynchronize(c->st));
+    }
+    s->h_stale = false;
+    return FSLIC_OK;
+}
+
 extern "C" int fslic_b200_crf_set_clusters(fslic_crf* c, int time, const fslic_cluster* h_clusters) {
     if (!h_clusters && c && c->N) return set_err(FSLIC_EINVAL, "NULL argument");
     CRF_FRAME(c, time, s);
@@ -2401,6 +2425,7 @@ extern "C" int fslic_b200_crf_set_clusters(fslic_crf* c, int time, const fslic_c
 extern "C" int fslic_b200_crf_get_clusters(fslic_crf* c, int time, fslic_cluster* h_out) {
     CrfSlot* s = nullptr;
     int rc = crf_frame(c, time, &s);
+    if (!rc) rc = crf_refresh_host(c, s);
     if (rc) return rc;
     if (c->N) memcpy(h_out, s->h_clusters.data(), sizeof(fslic_cluster) * c->N);
     return FSLIC_OK;
@@ -2413,6 +2438,7 @@ extern "C" int fslic_b200_crf_set_connectivity(fslic_crf* c, int time, int num_r
                                                const int32_t* h_neighbors) {
     CrfSlot* s = nullptr;
     int rc = crf_frame(c, time, &s);
+    if (!rc) rc = crf_refresh_host(c, s);
     if (rc) return rc;
     const int N = c->N;
     if (num_rows < 0 || num_rows > N) return set_err(FSLIC_EINVAL, "more adjacency lists than nodes");
@@ -2462,6 +2488,7 @@ extern "C" int fslic_b200_crf_get_connectivity(fslic_crf* c, int time, int32_t* 
                                                long long cap) {
     CrfSlot* s = nullptr;
     int rc = crf_frame(c, time, &s);
+    if (!rc) rc = crf_refresh_host(c, s);
     if (rc) return rc;
     if (h_offsets) memcpy(h_offsets, s->h_off.data(), sizeof(int32_t) * (c->N + 1));
     if (h_neighbors) {
@@ -2594,6 +2621,7 @@ extern "C" int fslic_b200_crf_inference(fslic_crf* c, unsigned long long max_ite
 extern "C" int fslic_b200_crf_spatial_pairwise_energy(fslic_crf* c, int time, int node_i, int node_j, float* out) {
     CRF_FRAME(c, time, s);
     if (node_i < 0 || node_j < 0 || node_i >= c->N || node_j >= c->N) return set_err(FSLIC_EINVAL, "node number is out of range");
+    { int rc = crf_refresh_host(c, s); if (rc) return rc; }
     if (node_i == node_j) {
         *out = 0.0f;
         return FSLIC_OK;
@@ -2614,6 +2642,9 @@ extern "C" int fslic_b200_crf_temporal_pairwise_energy(fslic_crf* c, int time, i
     if (rc) return rc;
     CRF_FRAME(c, time, s);
     if (node < 0 || node >= c->N || node >= other->N) return set_err(FSLIC_EINVAL, "node number is out of range");
+    rc = crf_refresh_host(c, s);
+    if (!rc) rc = crf_refresh_host(other, o);
+    if (rc) return rc;
     if (s == o) {
         *out = 0.0f;
         return FSLIC_OK;
@@ -2646,6 +2677,231 @@ extern "C" int fslic_b200_debug_expf_device(int device, uint32_t first, long lon
     if (!n) return FSLIC_OK;
     USE_DEVICE(device);
     k_expf_debug<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(first, n, d_out);
+    CK(cudaGetLastError());
+    return FSLIC_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The CRF fed from device memory (crf_feed.cuh).  Each entry point adopts `stream` the way inference does (waiting for
+// the CRF's previous stream if it differs) and only enqueues: labels, clusters, graphs and unaries never pass through
+// the host.  The host waits left are the frame-table upload every push makes and set_mask's 4-byte validity flag.
+// A device push marks the frame's host copies stale; crf_refresh_host brings them back for the host-side readers.
+
+// Switch the CRF to `stream`, waiting for the old one if it differs (as fslic_b200_crf_inference does)
+static int crf_adopt_stream(fslic_crf* c, void* stream) {
+    if ((cudaStream_t)stream != c->st) {
+        CK(cudaStreamSynchronize(c->st));
+        c->st = (cudaStream_t)stream;
+    }
+    return FSLIC_OK;
+}
+
+// The graph of `batch` label maps (fslic_b200_get_connectivity_batch's scratch) followed by their counts [batch][K] and
+// neighbour lists [batch][K][12].
+extern "C" size_t fslic_b200_crfdev_push_scratch_bytes(int K, int batch) {
+    const size_t graph = fslic_b200_connectivity_batch_scratch_bytes(K, batch);
+    if (graph == (size_t)-1) return graph;
+    if (K <= 0 || batch <= 0) return 256;
+    return align_up(graph, 256) + align_up((size_t)batch * K * 4, 256) + align_up((size_t)batch * K * CONN_MAX * 4, 256);
+}
+
+// A slot for a device push: from the pool or newly allocated, with room for 12 * N edges (the graph's cap), so the
+// steady state never reallocates.  The slot is not in the deque yet.
+static int crfdev_take_slot(fslic_crf* c, CrfSlot** out) {
+    const size_t N = (size_t)c->N, CN = (size_t)c->C * c->N, E = N * CONN_MAX;
+    CrfSlot* s;
+    if (!c->pool.empty()) {
+        s = c->pool.back();
+        c->pool.pop_back();
+    } else {
+        s = new (std::nothrow) CrfSlot();
+        if (!s) return set_err(FSLIC_ENOMEM, "out of host memory");
+        cudaError_t e = cudaSuccess;
+        if (e == cudaSuccess && N) e = cudaMalloc(&s->clusters, sizeof(fslic_cluster) * N);
+        if (e == cudaSuccess) e = cudaMalloc(&s->offsets, sizeof(int32_t) * (N + 1));
+        if (e == cudaSuccess && CN) e = cudaMalloc(&s->unary, sizeof(float) * CN);
+        if (e == cudaSuccess && CN) e = cudaMalloc(&s->q0, sizeof(float) * CN);
+        if (e == cudaSuccess && CN) e = cudaMalloc(&s->q1, sizeof(float) * CN);
+        if (e == cudaSuccess && CN) e = cudaMalloc(&s->msg, sizeof(float) * CN);
+        if (e == cudaSuccess && N) e = cudaMalloc(&s->tmp, sizeof(float) * 4 * N);
+        if (e != cudaSuccess) {
+            crf_free_slot(s);
+            return set_err(e == cudaErrorMemoryAllocation ? FSLIC_ENOMEM : FSLIC_ECUDA,
+                           std::string("cudaMalloc: ") + cudaGetErrorString(e));
+        }
+    }
+    if (s->edge_cap < E) {
+        cudaFree(s->nbr); cudaFree(s->e_sp); cudaFree(s->r_sp);
+        s->nbr = nullptr; s->e_sp = s->r_sp = nullptr; s->edge_cap = 0;
+        cudaError_t e = cudaMalloc(&s->nbr, sizeof(int32_t) * E);
+        if (e == cudaSuccess) e = cudaMalloc(&s->e_sp, sizeof(float) * E);
+        if (e == cudaSuccess) e = cudaMalloc(&s->r_sp, sizeof(float) * E);
+        if (e != cudaSuccess) {
+            c->pool.push_back(s);  // keeps its node buffers; edge_cap 0 makes the next push retry
+            return set_err(e == cudaErrorMemoryAllocation ? FSLIC_ENOMEM : FSLIC_ECUDA,
+                           std::string("cudaMalloc: ") + cudaGetErrorString(e));
+        }
+        s->edge_cap = E;
+    }
+    s->h_clusters.resize(N);  // sizes the host readers rely on; the contents are stale until refreshed
+    s->h_off.resize(N + 1);
+    s->h_stale = true;
+    *out = s;
+    return FSLIC_OK;
+}
+
+// Pushes `batch` frames; frame b is what push_slic_frame gives for label map d_labels[b] (int16 [H][W], labels outside
+// [0, K) ignored) and records d_clusters[b] ([K]): its records, its adjacency graph and unbiased unaries.  K must equal
+// the CRF's num_nodes.  Every argument is checked before anything is pushed (the host push_slic_frame pushes a blank
+// frame first and only then fails on a K mismatch).  times_out (host, [batch], may be NULL) receives the new times.
+extern "C" int fslic_b200_crfdev_push_label_frames(fslic_crf* c, int batch, int H, int W, int K, const uint16_t* d_labels,
+                                                   const fslic_cluster* d_clusters, void* d_scratch, size_t scratch_bytes,
+                                                   void* stream, int* times_out) {
+    if (!c) return set_err(FSLIC_EINVAL, "crf is NULL");
+    if (K != c->N) return set_err(FSLIC_EINVAL, "K must equal the CRF's num_nodes");
+    if (batch < 0 || H <= 0 || W <= 0 || K <= 0 || K > 65535) return set_err(FSLIC_EINVAL, "bad batch, H, W or K");
+    if (batch == 0) return FSLIC_OK;
+    if (!d_labels || !d_clusters || !d_scratch) return set_err(FSLIC_EINVAL, "NULL argument");
+    const size_t need = fslic_b200_crfdev_push_scratch_bytes(K, batch);
+    if (need == (size_t)-1) return set_err(FSLIC_EINVAL, "batch too large for one call");
+    if (scratch_bytes < need) return set_err(FSLIC_EINVAL, "scratch too small");
+    const int obits = bit_length(3ull * (unsigned long long)H * (unsigned long long)W);
+    if (obits + bit_length(batch - 1) > 64) return set_err(FSLIC_EINVAL, "batch * H * W too large");
+    USE_DEVICE(c->device);
+    { int rc = crf_adopt_stream(c, stream); if (rc) return rc; }
+    std::vector<CrfSlot*> slots;
+    for (int b = 0; b < batch; b++) {
+        CrfSlot* s = nullptr;
+        int rc = crfdev_take_slot(c, &s);
+        if (rc) {
+            for (CrfSlot* t : slots) c->pool.push_back(t);
+            return rc;
+        }
+        slots.push_back(s);
+    }
+    // the new frames join the table first, so the one host wait (the table upload) does not include this push's work
+    const int next_time0 = c->next_time;
+    for (CrfSlot* s : slots) {
+        s->time = c->next_time++;
+        c->frames.push_back(s);
+    }
+    int rc = crf_upload_table(c);
+    if (!rc) {
+        const size_t graph_bytes = align_up(fslic_b200_connectivity_batch_scratch_bytes(K, batch), 256);
+        unsigned char* p = static_cast<unsigned char*>(d_scratch);
+        int32_t* counts = reinterpret_cast<int32_t*>(p + graph_bytes);
+        uint32_t* nbrs = reinterpret_cast<uint32_t*>(p + graph_bytes + align_up((size_t)batch * K * 4, 256));
+        rc = fslic_b200_get_connectivity_batch(c->device, batch, H, W, K, d_labels, counts, nbrs, nullptr, d_scratch,
+                                               graph_bytes, stream);
+        const long long CN = (long long)c->C * K;
+        const float unbiased = logf((float)c->C);  // set_unbiased's constant, glibc's logf as on the host path
+        for (int b = 0; b < batch && !rc; b++) {
+            CrfSlot* s = slots[b];
+            k_feed_nodes<<<(int)grid_for(CN > K ? CN : K, c->device), 256, 0, c->st>>>(
+                d_clusters + (size_t)b * K, FeedFramePtrs{s->clusters, s->unary, s->q0, s->q1}, K, c->C, unbiased);
+            k_feed_csr<<<1, FEED_CSR_THREADS, 0, c->st>>>(counts + (size_t)b * K, nbrs + (size_t)b * K * CONN_MAX, K,
+                                                          s->offsets, s->nbr);
+            const cudaError_t e = cudaGetLastError();
+            if (e != cudaSuccess) rc = set_err(FSLIC_ECUDA, std::string("feed kernels: ") + cudaGetErrorString(e));
+        }
+    }
+    if (rc) {  // take the frames back out
+        for (int b = 0; b < batch; b++) {
+            c->pool.push_back(c->frames.back());
+            c->frames.pop_back();
+        }
+        c->next_time = next_time0;
+        crf_upload_table(c);
+        return rc;
+    }
+    if (times_out)
+        for (int b = 0; b < batch; b++) times_out[b] = slots[b]->time;
+    return FSLIC_OK;
+}
+
+// Look up frame `time`, switch to the CRF's device and adopt `stream`: the device setters never wait for it.
+#define CRFDEV_FRAME(c, time, s, stream)                                                              \
+    CrfSlot* s = nullptr;                                                                             \
+    { int rc__ = crf_frame(c, time, &s); if (rc__) return rc__; }                                     \
+    USE_DEVICE((c)->device);                                                                          \
+    { int rc__ = crf_adopt_stream(c, stream); if (rc__) return rc__; }
+
+// set_unary from device memory: float [C][N], copied on the stream
+extern "C" int fslic_b200_crfdev_set_unary(fslic_crf* c, int time, const float* d_unary, void* stream) {
+    CRFDEV_FRAME(c, time, s, stream);
+    const size_t CN = (size_t)c->C * c->N;
+    if (CN && !d_unary) return set_err(FSLIC_EINVAL, "NULL argument");
+    if (CN) CK(cudaMemcpyAsync(s->unary, d_unary, sizeof(float) * CN, cudaMemcpyDeviceToDevice, c->st));
+    return FSLIC_OK;
+}
+
+// set_proba from device memory: unary = -logf(p) with glibc's logf (glibc_logf.cuh), p float [C][N]
+extern "C" int fslic_b200_crfdev_set_proba(fslic_crf* c, int time, const float* d_proba, void* stream) {
+    CRFDEV_FRAME(c, time, s, stream);
+    const long long CN = (long long)c->C * c->N;
+    if (!CN) return FSLIC_OK;
+    if (!d_proba) return set_err(FSLIC_EINVAL, "NULL argument");
+    k_feed_proba<<<(int)grid_for(CN, c->device), 256, 0, c->st>>>(d_proba, s->unary, CN);
+    CK(cudaGetLastError());
+    return FSLIC_OK;
+}
+
+// set_mask from device memory: classes int32 [N], each in [0, C), checked on the device; the call waits for that one
+// flag and changes nothing if any class is out of range.  The two unary values are the host path's: fmaf, division
+// and glibc's logf in its order, on the host.
+extern "C" int fslic_b200_crfdev_set_mask(fslic_crf* c, int time, const int32_t* d_classes, float confidence, void* stream) {
+    CRFDEV_FRAME(c, time, s, stream);
+    const int C = c->C, N = c->N;
+    if (!N) return FSLIC_OK;
+    if (!d_classes) return set_err(FSLIC_EINVAL, "NULL argument");
+    int* d_bad = reinterpret_cast<int*>(c->d_scalar);
+    CK(cudaMemsetAsync(d_bad, 0, sizeof(int), c->st));
+    k_feed_mask_check<<<(int)grid_for(N, c->device), 256, 0, c->st>>>(d_classes, N, C, d_bad);
+    CK(cudaGetLastError());
+    int bad = 0;
+    CK(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, c->st));
+    CK(cudaStreamSynchronize(c->st));
+    if (bad) return set_err(FSLIC_EINVAL, "class index out of range");
+    const float lowest = 1.0f / (float)C;
+    const float active = fmaf(1.0f - lowest, confidence, lowest);
+    const float inactive = (1.0f - active) / (float)(C - 1);
+    const float active_unary = glogf::neg_logf(active), inactive_unary = glogf::neg_logf(inactive);
+    const long long CN = (long long)C * N;
+    k_feed_mask<<<(int)grid_for(CN, c->device), 256, 0, c->st>>>(d_classes, N, C, active_unary, inactive_unary, s->unary);
+    CK(cudaGetLastError());
+    return FSLIC_OK;
+}
+
+// get_inferred into device memory: q float [C][N], copied on the stream
+extern "C" int fslic_b200_crfdev_get_inferred(fslic_crf* c, int time, float* d_out, void* stream) {
+    CRFDEV_FRAME(c, time, s, stream);
+    const size_t CN = (size_t)c->C * c->N;
+    if (CN && !d_out) return set_err(FSLIC_EINVAL, "NULL argument");
+    if (CN) CK(cudaMemcpyAsync(d_out, c->cur ? s->q1 : s->q0, sizeof(float) * CN, cudaMemcpyDeviceToDevice, c->st));
+    return FSLIC_OK;
+}
+
+// The logf clone of glibc_logf.cuh over the bit patterns first .. first + n - 1 (wrapping), host and device compiles.
+__attribute__((target("fma"))) static void logf_host_fma(uint32_t first, long long n, float* out) {
+    for (long long i = 0; i < n; i++) out[i] = glogf::logf(gexpf::u2f(first + (uint32_t)i));
+}
+static void logf_host_generic(uint32_t first, long long n, float* out) {
+    for (long long i = 0; i < n; i++) out[i] = glogf::logf(gexpf::u2f(first + (uint32_t)i));
+}
+
+extern "C" int fslic_b200_debug_logf_host(uint32_t first, long long n, float* h_out) {
+    if (n < 0 || (n && !h_out)) return set_err(FSLIC_EINVAL, "bad buffer");
+    // both are exact (libm's fma is correctly rounded); the FMA instruction is only faster
+    if (__builtin_cpu_supports("fma")) logf_host_fma(first, n, h_out);
+    else logf_host_generic(first, n, h_out);
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_debug_logf_device(int device, uint32_t first, long long n, float* d_out, void* stream) {
+    if (n < 0 || (n && !d_out)) return set_err(FSLIC_EINVAL, "bad buffer");
+    if (!n) return FSLIC_OK;
+    USE_DEVICE(device);
+    k_logf_debug<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(first, n, d_out);
     CK(cudaGetLastError());
     return FSLIC_OK;
 }

@@ -343,6 +343,36 @@ int fslic_b200_crf_temporal_pairwise_energy(fslic_crf* crf, int time, int node, 
 int fslic_b200_debug_expf_host(uint32_t first, long long n, float* h_out);
 int fslic_b200_debug_expf_device(int device, uint32_t first, long long n, float* d_out, void* stream);
 
+/* ---- The CRF fed from device memory (fast_slic_b200/csrc/crf_feed.cuh).  A separate prefix from the reference's
+ * fslic_b200_crf_* surface above.  All d_* buffers are device memory on the CRF's device.  Each call adopts `stream`
+ * like fslic_b200_crf_inference (waiting for the CRF's previous stream if it differs) and enqueues its work there
+ * without waiting for it; labels, clusters, graphs and unaries never pass through the host.  Each frame equals what the
+ * host path stores for the same input, bit for bit.  After a device push, the host-side readers of a frame
+ * (get_clusters, get_connectivity, set_connectivity, the pairwise energies) first wait for the stream and download the
+ * frame's records and adjacency lists once. */
+/* Scratch bytes fslic_b200_crfdev_push_label_frames needs for `batch` label maps with K labels; (size_t)-1 if no
+ * single call can take that batch. */
+size_t fslic_b200_crfdev_push_scratch_bytes(int K, int batch);
+/* Pushes `batch` frames.  Frame b holds d_clusters[b] ([K] records, converted as push_slic_frame converts them: y, x,
+ * r, g, b and num_members truncated to int32 the way x86 numpy does, with INT_MIN for NaN, inf and out-of-range values),
+ * the adjacency graph of d_labels[b] (int16 [H][W]; labels outside [0, K) ignored), and unbiased unaries.  K must
+ * equal num_nodes.  Bad arguments are refused before anything is pushed.  times_out [batch] (host, may be NULL)
+ * receives the new frames' times.  The one host wait is the frame-table upload every push makes; it covers work
+ * enqueued before the call, not this push's kernels. */
+int fslic_b200_crfdev_push_label_frames(fslic_crf* crf, int batch, int H, int W, int K, const uint16_t* d_labels,
+                                        const fslic_cluster* d_clusters, void* d_scratch, size_t scratch_bytes,
+                                        void* stream, int* times_out);
+int fslic_b200_crfdev_set_unary(fslic_crf* crf, int time, const float* d_unary, void* stream);
+int fslic_b200_crfdev_set_proba(fslic_crf* crf, int time, const float* d_proba, void* stream); /* -logf(p) */
+/* classes int32 [N] are checked on the device; the call waits for that 4-byte flag and changes nothing (FSLIC_EINVAL)
+ * if any class is outside [0, C) */
+int fslic_b200_crfdev_set_mask(fslic_crf* crf, int time, const int32_t* d_classes, float confidence, void* stream);
+int fslic_b200_crfdev_get_inferred(fslic_crf* crf, int time, float* d_out, void* stream);
+
+/* glibc's logf as the device feed evaluates it (fast_slic_b200/csrc/glibc_logf.cuh), like the expf pair above. */
+int fslic_b200_debug_logf_host(uint32_t first, long long n, float* h_out);
+int fslic_b200_debug_logf_device(int device, uint32_t first, long long n, float* d_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -67,6 +67,7 @@ def lib():
         L.orcl_crf_inference.argtypes = [C.c_int, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.POINTER(Params), C.c_longlong, C.c_void_p]
         L.orcl_expf_range.argtypes = [C.c_uint32, C.c_longlong, C.c_void_p]
+        L.orcl_logf_range.argtypes = [C.c_uint32, C.c_longlong, C.c_void_p]
         _lib = L
     return _lib
 
@@ -75,6 +76,13 @@ def glibc_expf_range(first, n):
     """glibc's expf over the float bit patterns first .. first + n - 1."""
     out = np.empty(n, np.float32)
     lib().orcl_expf_range(first, n, _vp(out))
+    return out
+
+
+def glibc_logf_range(first, n):
+    """glibc's logf over the float bit patterns first .. first + n - 1."""
+    out = np.empty(n, np.float32)
+    lib().orcl_logf_range(first, n, _vp(out))
     return out
 
 

@@ -142,3 +142,12 @@ void orcl_expf_range(uint32_t first, long long n, float* out) {
         out[i] = expf(v.f);
     }
 }
+
+/* glibc's logf over the bit patterns first .. first + n - 1 */
+void orcl_logf_range(uint32_t first, long long n, float* out) {
+    for (long long i = 0; i < n; i++) {
+        union { uint32_t u; float f; } v;
+        v.u = first + (uint32_t)i;
+        out[i] = logf(v.f);
+    }
+}
