@@ -12,12 +12,9 @@
 #include <string>
 #include <vector>
 
-#include <cub/device/device_radix_sort.cuh>  // library sort for the adjacency-graph utility only (not on the hot path)
-
 #include "assign.cuh"
 #include "assign5.cuh"
-#include "graph.cuh"
-#include "graph_batch.cuh"
+#include "capi_common.h"
 #include "realdist.cuh"
 #include "lsc.cuh"
 #include "crf.cuh"
@@ -39,39 +36,12 @@ typedef void (*assign5_fn)(const AssignParams, const CUtensorMap, const CUtensor
                            const int*, unsigned long long*, const uint16_t*, fslic_cluster*, CInfo*, int*, unsigned int*);
 static assign5_fn pick_assign5(int TS, bool update, int tps, bool fuse = false);
 
+// The one message fslic_b200_last_error() returns, for the entry points of every translation unit
 static thread_local std::string g_err;
-static int set_err(int code, const std::string& msg) {
+int set_err(int code, const std::string& msg) {
     g_err = msg;
     return code;
 }
-// Every entry point runs on the context's device and puts the caller's current device back on return
-// (a single-process multi-GPU PyTorch program must not find its current device changed behind its back).
-struct DeviceGuard {
-    int prev = -1;
-    bool changed = false;
-    cudaError_t err = cudaSuccess;
-    explicit DeviceGuard(int dev) {
-        err = cudaGetDevice(&prev);
-        if (err == cudaSuccess && prev != dev) {
-            err = cudaSetDevice(dev);
-            changed = err == cudaSuccess;
-        }
-    }
-    ~DeviceGuard() {
-        if (changed) cudaSetDevice(prev);
-    }
-};
-#define USE_DEVICE(dev)                                                                               \
-    DeviceGuard dev_guard__(dev);                                                                     \
-    if (dev_guard__.err != cudaSuccess)                                                               \
-        return set_err(FSLIC_ECUDA, std::string("cudaSetDevice: ") + cudaGetErrorString(dev_guard__.err))
-
-#define CK(call)                                                                                      \
-    do {                                                                                              \
-        cudaError_t e__ = (call);                                                                     \
-        if (e__ != cudaSuccess)                                                                       \
-            return set_err(FSLIC_ECUDA, std::string(#call) + ": " + cudaGetErrorString(e__));         \
-    } while (0)
 
 // What the host enqueued for one assign pass (fslic_b200_debug_dispatch): kernel 5 = TMA-staged, 4 = LDG warp tiles,
 // 0 = generic, 10 / 11 / 12 = float-distance variant 0 / 1 / 2, 13 = preemptive, 14 = LSC, -1 = none yet.  Workers
@@ -1982,205 +1952,6 @@ extern "C" int fslic_b200_wait(fslic_ctx* c) {
     return FSLIC_OK;
 }
 
-// ---- consumers of the label map (SURVEY.md 8(f) rows 1-2): stateless, device pointers, caller-provided scratch ------
-static uint32_t conn_table_size(int K) {
-    uint32_t t = 4096;
-    while (t < 32u * (uint32_t)K) t <<= 1;  // a superpixel map has ~3 distinct adjacent pairs per label
-    return t;
-}
-static size_t conn_sort_temp_bytes(uint32_t T) {
-    size_t bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                    (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)T);
-    return bytes;
-}
-
-// grid cap of the grid-stride kernels of the context-free entry points below: 16 CTAs per SM of `device`
-static long grid_stride_cap(int device) {
-    int sms = 0;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms <= 0) sms = 1;
-    return 16L * sms;
-}
-
-extern "C" size_t fslic_b200_connectivity_scratch_bytes(int K) {
-    if (K <= 0) return 256;
-    const size_t T = conn_table_size(K);
-    return align_up(T * 4, 256) * 2 + align_up(T * 8, 256) * 2 + align_up(conn_sort_temp_bytes((uint32_t)T), 256) + 256;
-}
-
-extern "C" int fslic_b200_get_connectivity(int device, int H, int W, int K, const uint16_t* d_labels, int32_t* d_counts,
-                                           uint32_t* d_neighbors, void* d_scratch, size_t scratch_bytes, void* stream) {
-    if (H <= 0 || W <= 0 || K <= 0 || K > 65535) return set_err(FSLIC_EINVAL, "bad H, W or K");
-    if (!d_labels || !d_counts || !d_neighbors || !d_scratch) return set_err(FSLIC_EINVAL, "NULL argument");
-    if (scratch_bytes < fslic_b200_connectivity_scratch_bytes(K)) return set_err(FSLIC_EINVAL, "scratch too small");
-    USE_DEVICE(device);
-    cudaStream_t st = (cudaStream_t)stream;
-    const uint32_t T = conn_table_size(K);
-    unsigned char* p = static_cast<unsigned char*>(d_scratch);
-    uint32_t* tkey = reinterpret_cast<uint32_t*>(p); p += align_up((size_t)T * 4, 256);
-    uint32_t* skey = reinterpret_cast<uint32_t*>(p); p += align_up((size_t)T * 4, 256);
-    unsigned long long* tord = reinterpret_cast<unsigned long long*>(p); p += align_up((size_t)T * 8, 256);
-    unsigned long long* sord = reinterpret_cast<unsigned long long*>(p); p += align_up((size_t)T * 8, 256);
-    size_t temp_bytes = conn_sort_temp_bytes(T);
-    void* temp = p; p += align_up(temp_bytes, 256);
-    int* overflow = reinterpret_cast<int*>(p);
-    CK(cudaMemsetAsync(tkey, 0xff, (size_t)T * 4, st));
-    CK(cudaMemsetAsync(tord, 0xff, (size_t)T * 8, st));
-    CK(cudaMemsetAsync(overflow, 0, 4, st));
-    CK(cudaMemsetAsync(d_counts, 0, (size_t)K * 4, st));
-    CK(cudaMemsetAsync(d_neighbors, 0, (size_t)K * CONN_MAX * 4, st));
-    if (H > 1 && W > 1) {
-        const long n = (long)(H - 1) * (W - 1);
-        long blocks = (n + 255) / 256;
-        const long cap = grid_stride_cap(device);
-        if (blocks > cap) blocks = cap;
-        k_conn_discover<<<(int)blocks, 256, 0, st>>>(d_labels, H, W, K, tkey, tord, T - 1, overflow);
-        int h_overflow = 0;
-        CK(cudaMemcpyAsync(&h_overflow, overflow, 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        if (h_overflow) {
-            k_conn_scan<<<1, 32, 0, st>>>(d_labels, H, W, K, d_counts, d_neighbors);
-        } else {
-            if (cub::DeviceRadixSort::SortPairs(temp, temp_bytes, tord, sord, tkey, skey, (int)T, 0, 64, st) != cudaSuccess)
-                return set_err(FSLIC_ECUDA, "radix sort of the pair table failed");
-            k_conn_walk<<<1, 32, 0, st>>>(sord, skey, T, K, d_counts, d_neighbors);
-        }
-    }
-    CK(cudaGetLastError());
-    return FSLIC_OK;
-}
-
-extern "C" int fslic_b200_get_mask_density(int device, int H, int W, int K, const fslic_cluster* d_clusters,
-                                           const uint16_t* d_labels, const uint8_t* d_mask, uint8_t* d_densities,
-                                           int32_t* d_scratch, void* stream) {
-    if (H <= 0 || W <= 0 || K <= 0 || K > 65535) return set_err(FSLIC_EINVAL, "bad H, W or K");
-    if (!d_clusters || !d_labels || !d_mask || !d_densities || !d_scratch) return set_err(FSLIC_EINVAL, "NULL argument");
-    USE_DEVICE(device);
-    cudaStream_t st = (cudaStream_t)stream;
-    const long n = (long)H * W;
-    CK(cudaMemsetAsync(d_scratch, 0, (size_t)K * 4, st));
-    long blocks = (n + 255) / 256;
-    const long cap = grid_stride_cap(device);
-    if (blocks > cap) blocks = cap;
-    k_mask_sum<<<(int)blocks, 256, 0, st>>>(d_labels, d_mask, n, K, d_scratch);
-    k_density_final<<<ceil_div(K, 256), 256, 0, st>>>(d_scratch, d_clusters, K, d_densities);
-    CK(cudaGetLastError());
-    return FSLIC_OK;
-}
-
-extern "C" int fslic_b200_cluster_density_to_mask(int device, int H, int W, int K, const uint16_t* d_labels,
-                                                  const uint8_t* d_densities, uint8_t* d_result, void* stream) {
-    if (H <= 0 || W <= 0 || K <= 0 || K > 65535) return set_err(FSLIC_EINVAL, "bad H, W or K");
-    if (!d_labels || !d_densities || !d_result) return set_err(FSLIC_EINVAL, "NULL argument");
-    USE_DEVICE(device);
-    const long n = (long)H * W;
-    long blocks = (n + 255) / 256;
-    const long cap = grid_stride_cap(device);
-    if (blocks > cap) blocks = cap;
-    k_density_broadcast<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(d_labels, d_densities, n, K, d_result);
-    CK(cudaGetLastError());
-    return FSLIC_OK;
-}
-
-// ---- the same consumers over a batch of label maps (graph_batch.cuh): stateless, asynchronous, never synchronise ----
-static int bit_length(unsigned long long v) {
-    int n = 0;
-    for (; v; v >>= 1) n++;
-    return n;
-}
-static size_t connb_sort_temp_bytes(long long items, int end_bit) {
-    size_t bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                    (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)items, 0, end_bit);
-    return bytes;
-}
-static long grid_for(long items, int device) {
-    long blocks = (items + 255) / 256;
-    const long cap = grid_stride_cap(device);
-    return blocks < 1 ? 1 : (blocks > cap ? cap : blocks);
-}
-
-// Key and order tables, their sorted copies, the sort's temporary storage (sized for all 64 key bits, an upper bound
-// of what a call sorts) and the per-image overflow flags.
-extern "C" size_t fslic_b200_connectivity_batch_scratch_bytes(int K, int batch) {
-    if (K <= 0 || batch <= 0) return 256;
-    if (K > 65535) return (size_t)-1;
-    const long long slots = (long long)conn_table_size(K) * batch;
-    if (slots > INT_MAX) return (size_t)-1;  // more than one radix sort takes: the call refuses such a batch
-    return align_up((size_t)slots * 4, 256) * 2 + align_up((size_t)slots * 8, 256) * 2 +
-           align_up(connb_sort_temp_bytes(slots, 64), 256) + align_up((size_t)batch * 4, 256);
-}
-
-extern "C" int fslic_b200_get_connectivity_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels,
-                                                 int32_t* d_counts, uint32_t* d_neighbors, int32_t* d_replayed,
-                                                 void* d_scratch, size_t scratch_bytes, void* stream) {
-    if (batch < 0 || H <= 0 || W <= 0 || K <= 0 || K > 65535) return set_err(FSLIC_EINVAL, "bad batch, H, W or K");
-    if (batch == 0) return FSLIC_OK;
-    if (!d_labels || !d_counts || !d_neighbors || !d_scratch) return set_err(FSLIC_EINVAL, "NULL argument");
-    const uint32_t T = conn_table_size(K);
-    const long long slots = (long long)T * batch;
-    if (slots > INT_MAX) return set_err(FSLIC_EINVAL, "batch too large for one call: the pair tables exceed 2^31 slots");
-    const int obits = bit_length(3ull * (unsigned long long)H * (unsigned long long)W), bits = obits + bit_length(batch - 1);
-    if (bits > 64) return set_err(FSLIC_EINVAL, "batch * H * W too large");
-    USE_DEVICE(device);
-    if (scratch_bytes < fslic_b200_connectivity_batch_scratch_bytes(K, batch)) return set_err(FSLIC_EINVAL, "scratch too small");
-    cudaStream_t st = (cudaStream_t)stream;
-    unsigned char* p = static_cast<unsigned char*>(d_scratch);
-    uint32_t* tkey = reinterpret_cast<uint32_t*>(p); p += align_up((size_t)slots * 4, 256);
-    uint32_t* skey = reinterpret_cast<uint32_t*>(p); p += align_up((size_t)slots * 4, 256);
-    unsigned long long* tord = reinterpret_cast<unsigned long long*>(p); p += align_up((size_t)slots * 8, 256);
-    unsigned long long* sord = reinterpret_cast<unsigned long long*>(p); p += align_up((size_t)slots * 8, 256);
-    size_t temp_bytes = align_up(connb_sort_temp_bytes(slots, 64), 256);
-    if (connb_sort_temp_bytes(slots, bits) > temp_bytes) return set_err(FSLIC_ECUDA, "radix sort temporary storage");
-    void* temp = p; p += temp_bytes;
-    int* overflow = reinterpret_cast<int*>(p);
-    // the walk's shared memory: u8 counts of the K labels + the staged chunk; opted in once per device for any K
-    const int smem = ((K + 15) & ~15) + CONNB_CHUNK * 4, smem_max = 65536 + CONNB_CHUNK * 4;
-    static bool walk_smem_set[64] = {};
-    if (device < 0 || device >= 64 || !walk_smem_set[device]) {
-        CK(cudaFuncSetAttribute(k_connb_walk, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-        if (device >= 0 && device < 64) walk_smem_set[device] = true;
-    }
-    k_connb_init<<<(int)grid_for(slots, device), 256, 0, st>>>(tkey, tord, slots, bit_length(T) - 1, obits, batch, overflow);
-    const long n = (long)batch * (H - 1) * (W - 1);
-    if (n > 0)
-        k_connb_discover<<<(int)grid_for(n, device), 256, 0, st>>>(d_labels, batch, H, W, K, tkey, tord, T, obits, overflow);
-    if (cub::DeviceRadixSort::SortPairs(temp, temp_bytes, tord, sord, tkey, skey, (int)slots, 0, bits, st) != cudaSuccess)
-        return set_err(FSLIC_ECUDA, "radix sort of the pair tables failed");
-    k_connb_walk<<<batch, 256, smem, st>>>(skey, T, d_labels, H, W, K, overflow, d_counts, d_neighbors, d_replayed);
-    CK(cudaGetLastError());
-    return FSLIC_OK;
-}
-
-extern "C" int fslic_b200_get_mask_density_batch(int device, int batch, int H, int W, int K, const fslic_cluster* d_clusters,
-                                                 const uint16_t* d_labels, const uint8_t* d_masks, uint8_t* d_densities,
-                                                 int32_t* d_scratch, void* stream) {
-    if (batch < 0 || H <= 0 || W <= 0 || K <= 0 || K > 65535) return set_err(FSLIC_EINVAL, "bad batch, H, W or K");
-    if (batch == 0) return FSLIC_OK;
-    if (!d_clusters || !d_labels || !d_masks || !d_densities || !d_scratch) return set_err(FSLIC_EINVAL, "NULL argument");
-    USE_DEVICE(device);
-    cudaStream_t st = (cudaStream_t)stream;
-    const long n = (long)H * W, nk = (long)batch * K;
-    CK(cudaMemsetAsync(d_scratch, 0, (size_t)nk * 4, st));
-    k_mask_sum_batch<<<(int)grid_for(n * batch, device), 256, 0, st>>>(d_labels, d_masks, n, batch, K, d_scratch);
-    k_density_final_batch<<<(int)grid_for(nk, device), 256, 0, st>>>(d_scratch, d_clusters, nk, d_densities);
-    CK(cudaGetLastError());
-    return FSLIC_OK;
-}
-
-extern "C" int fslic_b200_cluster_density_to_mask_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels,
-                                                        const uint8_t* d_densities, uint8_t* d_result, void* stream) {
-    if (batch < 0 || H <= 0 || W <= 0 || K <= 0 || K > 65535) return set_err(FSLIC_EINVAL, "bad batch, H, W or K");
-    if (batch == 0) return FSLIC_OK;
-    if (!d_labels || !d_densities || !d_result) return set_err(FSLIC_EINVAL, "NULL argument");
-    USE_DEVICE(device);
-    const long n = (long)H * W;
-    k_density_broadcast_batch<<<(int)grid_for(n * batch, device), 256, 0, (cudaStream_t)stream>>>(d_labels, d_densities, n,
-                                                                                                   batch, K, d_result);
-    CK(cudaGetLastError());
-    return FSLIC_OK;
-}
-
 // ---------------------------------------------------------------------------------------------------------------------
 // SimpleCRF (src/simple-crf.{h,hpp,cpp}; csimple_crf.pyx).  The frames live in a deque in time order, exactly like the
 // reference's; each owns its device buffers (crf.cuh) plus host copies of its clusters and adjacency lists, which the
@@ -2218,6 +1989,33 @@ static void crf_free_slot(CrfSlot* s) {
     cudaFree(s->clusters); cudaFree(s->offsets); cudaFree(s->nbr); cudaFree(s->e_sp); cudaFree(s->r_sp);
     cudaFree(s->unary); cudaFree(s->q0); cudaFree(s->q1); cudaFree(s->msg); cudaFree(s->tmp);
     delete s;
+}
+
+// A slot from the pool, or a new one with its node buffers allocated; the edge buffers are left to the caller.
+static int crf_take_slot(fslic_crf* c, CrfSlot** out) {
+    if (!c->pool.empty()) {
+        *out = c->pool.back();
+        c->pool.pop_back();
+        return FSLIC_OK;
+    }
+    const size_t N = (size_t)c->N, CN = (size_t)c->C * c->N;
+    CrfSlot* s = new (std::nothrow) CrfSlot();
+    if (!s) return set_err(FSLIC_ENOMEM, "out of host memory");
+    cudaError_t e = cudaSuccess;
+    if (e == cudaSuccess && N) e = cudaMalloc(&s->clusters, sizeof(fslic_cluster) * N);
+    if (e == cudaSuccess) e = cudaMalloc(&s->offsets, sizeof(int32_t) * (N + 1));
+    if (e == cudaSuccess && CN) e = cudaMalloc(&s->unary, sizeof(float) * CN);
+    if (e == cudaSuccess && CN) e = cudaMalloc(&s->q0, sizeof(float) * CN);
+    if (e == cudaSuccess && CN) e = cudaMalloc(&s->q1, sizeof(float) * CN);
+    if (e == cudaSuccess && CN) e = cudaMalloc(&s->msg, sizeof(float) * CN);
+    if (e == cudaSuccess && N) e = cudaMalloc(&s->tmp, sizeof(float) * 4 * N);
+    if (e != cudaSuccess) {
+        crf_free_slot(s);
+        return set_err(e == cudaErrorMemoryAllocation ? FSLIC_ENOMEM : FSLIC_ECUDA,
+                       std::string("cudaMalloc: ") + cudaGetErrorString(e));
+    }
+    *out = s;
+    return FSLIC_OK;
 }
 
 #define CKA(call)                                                                                     \
@@ -2325,26 +2123,7 @@ extern "C" int fslic_b200_crf_push_frame(fslic_crf* c, int* time_out) {
     CK(cudaStreamSynchronize(c->st));
     const size_t N = (size_t)c->N, CN = (size_t)c->C * c->N;
     CrfSlot* s;
-    if (!c->pool.empty()) {
-        s = c->pool.back();
-        c->pool.pop_back();
-    } else {
-        s = new (std::nothrow) CrfSlot();
-        if (!s) return set_err(FSLIC_ENOMEM, "out of host memory");
-        cudaError_t e = cudaSuccess;
-        if (e == cudaSuccess && N) e = cudaMalloc(&s->clusters, sizeof(fslic_cluster) * N);
-        if (e == cudaSuccess) e = cudaMalloc(&s->offsets, sizeof(int32_t) * (N + 1));
-        if (e == cudaSuccess && CN) e = cudaMalloc(&s->unary, sizeof(float) * CN);
-        if (e == cudaSuccess && CN) e = cudaMalloc(&s->q0, sizeof(float) * CN);
-        if (e == cudaSuccess && CN) e = cudaMalloc(&s->q1, sizeof(float) * CN);
-        if (e == cudaSuccess && CN) e = cudaMalloc(&s->msg, sizeof(float) * CN);
-        if (e == cudaSuccess && N) e = cudaMalloc(&s->tmp, sizeof(float) * 4 * N);
-        if (e != cudaSuccess) {
-            crf_free_slot(s);
-            return set_err(e == cudaErrorMemoryAllocation ? FSLIC_ENOMEM : FSLIC_ECUDA,
-                           std::string("cudaMalloc: ") + cudaGetErrorString(e));
-        }
-    }
+    { int rc = crf_take_slot(c, &s); if (rc) return rc; }
     // SimpleCRFFrame::SimpleCRFFrame (simple-crf.hpp:29-33): value-initialised clusters with num_members = 1, empty
     // adjacency lists, unaries and q zero
     fslic_cluster blank;
@@ -2656,20 +2435,27 @@ extern "C" int fslic_b200_crf_temporal_pairwise_energy(fslic_crf* c, int time, i
     return FSLIC_OK;
 }
 
-// The expf clone of glibc_expf.cuh over the bit patterns first .. first + n - 1 (wrapping), host and device compiles.
-__attribute__((target("fma"))) static void expf_host_fma(uint32_t first, long long n, float* out) {
-    for (long long i = 0; i < n; i++) out[i] = gexpf::expf(gexpf::u2f(first + (uint32_t)i));
+// A glibc clone (glibc_expf.cuh, glibc_logf.cuh) over the bit patterns first .. first + n - 1 (wrapping) on the host,
+// with the FMA instruction where the CPU has it.  Both compiles are exact (libm's fma is correctly rounded); the FMA
+// instruction is only faster.
+template <float (*fn)(float)>
+static inline __attribute__((always_inline)) void host_over_bits(uint32_t first, long long n, float* out) {
+    for (long long i = 0; i < n; i++) out[i] = fn(gexpf::u2f(first + (uint32_t)i));
 }
-static void expf_host_generic(uint32_t first, long long n, float* out) {
-    for (long long i = 0; i < n; i++) out[i] = gexpf::expf(gexpf::u2f(first + (uint32_t)i));
+template <float (*fn)(float)>
+__attribute__((target("fma"))) static void host_over_bits_fma(uint32_t first, long long n, float* out) {
+    host_over_bits<fn>(first, n, out);
+}
+template <float (*fn)(float)>
+static int debug_host_over_bits(uint32_t first, long long n, float* h_out) {
+    if (n < 0 || (n && !h_out)) return set_err(FSLIC_EINVAL, "bad buffer");
+    if (__builtin_cpu_supports("fma")) host_over_bits_fma<fn>(first, n, h_out);
+    else host_over_bits<fn>(first, n, h_out);
+    return FSLIC_OK;
 }
 
 extern "C" int fslic_b200_debug_expf_host(uint32_t first, long long n, float* h_out) {
-    if (n < 0 || (n && !h_out)) return set_err(FSLIC_EINVAL, "bad buffer");
-    // both are exact (libm's fma is correctly rounded); the FMA instruction is only faster
-    if (__builtin_cpu_supports("fma")) expf_host_fma(first, n, h_out);
-    else expf_host_generic(first, n, h_out);
-    return FSLIC_OK;
+    return debug_host_over_bits<gexpf::expf>(first, n, h_out);
 }
 
 extern "C" int fslic_b200_debug_expf_device(int device, uint32_t first, long long n, float* d_out, void* stream) {
@@ -2708,28 +2494,9 @@ extern "C" size_t fslic_b200_crfdev_push_scratch_bytes(int K, int batch) {
 // A slot for a device push: from the pool or newly allocated, with room for 12 * N edges (the graph's cap), so the
 // steady state never reallocates.  The slot is not in the deque yet.
 static int crfdev_take_slot(fslic_crf* c, CrfSlot** out) {
-    const size_t N = (size_t)c->N, CN = (size_t)c->C * c->N, E = N * CONN_MAX;
+    const size_t N = (size_t)c->N, E = N * CONN_MAX;
     CrfSlot* s;
-    if (!c->pool.empty()) {
-        s = c->pool.back();
-        c->pool.pop_back();
-    } else {
-        s = new (std::nothrow) CrfSlot();
-        if (!s) return set_err(FSLIC_ENOMEM, "out of host memory");
-        cudaError_t e = cudaSuccess;
-        if (e == cudaSuccess && N) e = cudaMalloc(&s->clusters, sizeof(fslic_cluster) * N);
-        if (e == cudaSuccess) e = cudaMalloc(&s->offsets, sizeof(int32_t) * (N + 1));
-        if (e == cudaSuccess && CN) e = cudaMalloc(&s->unary, sizeof(float) * CN);
-        if (e == cudaSuccess && CN) e = cudaMalloc(&s->q0, sizeof(float) * CN);
-        if (e == cudaSuccess && CN) e = cudaMalloc(&s->q1, sizeof(float) * CN);
-        if (e == cudaSuccess && CN) e = cudaMalloc(&s->msg, sizeof(float) * CN);
-        if (e == cudaSuccess && N) e = cudaMalloc(&s->tmp, sizeof(float) * 4 * N);
-        if (e != cudaSuccess) {
-            crf_free_slot(s);
-            return set_err(e == cudaErrorMemoryAllocation ? FSLIC_ENOMEM : FSLIC_ECUDA,
-                           std::string("cudaMalloc: ") + cudaGetErrorString(e));
-        }
-    }
+    { int rc = crf_take_slot(c, &s); if (rc) return rc; }
     if (s->edge_cap < E) {
         cudaFree(s->nbr); cudaFree(s->e_sp); cudaFree(s->r_sp);
         s->nbr = nullptr; s->e_sp = s->r_sp = nullptr; s->edge_cap = 0;
@@ -2881,20 +2648,8 @@ extern "C" int fslic_b200_crfdev_get_inferred(fslic_crf* c, int time, float* d_o
     return FSLIC_OK;
 }
 
-// The logf clone of glibc_logf.cuh over the bit patterns first .. first + n - 1 (wrapping), host and device compiles.
-__attribute__((target("fma"))) static void logf_host_fma(uint32_t first, long long n, float* out) {
-    for (long long i = 0; i < n; i++) out[i] = glogf::logf(gexpf::u2f(first + (uint32_t)i));
-}
-static void logf_host_generic(uint32_t first, long long n, float* out) {
-    for (long long i = 0; i < n; i++) out[i] = glogf::logf(gexpf::u2f(first + (uint32_t)i));
-}
-
 extern "C" int fslic_b200_debug_logf_host(uint32_t first, long long n, float* h_out) {
-    if (n < 0 || (n && !h_out)) return set_err(FSLIC_EINVAL, "bad buffer");
-    // both are exact (libm's fma is correctly rounded); the FMA instruction is only faster
-    if (__builtin_cpu_supports("fma")) logf_host_fma(first, n, h_out);
-    else logf_host_generic(first, n, h_out);
-    return FSLIC_OK;
+    return debug_host_over_bits<glogf::logf>(first, n, h_out);
 }
 
 extern "C" int fslic_b200_debug_logf_device(int device, uint32_t first, long long n, float* d_out, void* stream) {

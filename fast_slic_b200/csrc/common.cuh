@@ -7,6 +7,7 @@
 #include "../../include/fslic_b200.h"
 
 #define FSLIC_FULL 0xffffffffu
+#define CONN_MAX 12  // neighbours per label in the adjacency graph (max_conn, fast-slic.cpp:17)
 
 // Out-of-window entries of the spatial patch.  Every in-window distance must stay below it and
 // BIGSP + 765 (max colour SAD) must stay below 65536 so `d * 65536 + rank` never wraps.

@@ -5,7 +5,6 @@
 #include <stdint.h>
 #include <cub/block/block_scan.cuh>
 #include "common.cuh"
-#include "graph.cuh"
 #include "glibc_logf.cuh"
 
 // numpy's float64 -> int32 cast on x86 (cvttsd2si): truncation, and INT_MIN for NaN, ±inf and anything whose truncation

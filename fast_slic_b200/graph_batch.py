@@ -1,6 +1,7 @@
 """Batched consumers of label maps: the adjacency graph, mask density and density broadcast of every image of a batch
-(csrc/graph_batch.cuh), each image equal to what SlicModel.get_connectivity / get_mask_density /
-broadcast_density_to_mask give for it alone.  No counterpart in the reference, which has no batch API.
+(csrc/graph.cuh), each image equal to what the reference's fast_slic_get_connectivity / fast_slic_get_mask_density /
+fast_slic_cluster_density_to_mask give for it alone.  The reference has no batch API; SlicModel.get_connectivity /
+get_mask_density / broadcast_density_to_mask, its single-image calls, are batches of one here.
 
 Cuda tensors in give cuda tensors out on the same device, enqueued on that device's current stream with no
 synchronisation (a CUDA graph can capture them); numpy arrays in give numpy arrays out.  Arguments are checked before

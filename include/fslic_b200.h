@@ -185,7 +185,8 @@ int fslic_b200_enforce_connectivity(fslic_ctx* ctx, uint16_t* d_labels, int batc
 /* == fast_slic_get_connectivity (src/fast-slic.cpp:16-78; cfast_slic.pyx:262-270): the superpixel adjacency graph of
  *    one label map d_labels u16[H*W] -> d_counts int32[K], d_neighbors u32[K*12] (row k: the first d_counts[k] entries,
  *    in the order the reference's raster scan links them; at most 12 per label, like the reference).  Stateless:
- *    d_scratch must hold fslic_b200_connectivity_scratch_bytes(K) bytes.  Synchronises `stream` once. */
+ *    d_scratch must hold fslic_b200_connectivity_scratch_bytes(K) bytes (= fslic_b200_connectivity_batch_scratch_bytes(K,
+ *    1)).  Asynchronous on `stream`. */
 size_t fslic_b200_connectivity_scratch_bytes(int K);
 int fslic_b200_get_connectivity(int device, int H, int W, int K, const uint16_t* d_labels, int32_t* d_counts,
                                 uint32_t* d_neighbors, void* d_scratch, size_t scratch_bytes, void* stream);

@@ -82,8 +82,10 @@ def _table_slots(K):
 def test_batch_scratch_grows_with_batch_and_components():
     from fast_slic_b200 import _lib
     f = _lib.lib().fslic_b200_connectivity_batch_scratch_bytes
+    single = _lib.lib().fslic_b200_connectivity_scratch_bytes
     assert f(0, 4) == 256 and f(10, 0) == 256
     for K in (1, 128, 129, 1600, 65533):
+        assert single(K) == f(K, 1), K
         prev = 0
         for B in (1, 2, 3, 32, 256):
             n = f(K, B)

@@ -391,6 +391,21 @@ def test_graph_and_density_consumers(checker, H, W, K, kind, msf):
         m.get_knn_connectivity(lab, 4)
 
 
+@pytest.mark.parametrize("H,W", [(0, 40), (40, 0)])
+def test_graph_and_density_consumers_refuse_an_empty_map(H, W):
+    """A label map without rows or columns is refused by all three single-image SlicModel methods."""
+    from fast_slic_b200 import SlicModel
+    K = 10
+    m = SlicModel(K)
+    lab = np.zeros((H, W), np.int16)
+    with pytest.raises(ValueError):
+        m.get_connectivity(lab)
+    with pytest.raises(ValueError):
+        m.get_mask_density(np.zeros((H, W), np.uint8), lab)
+    with pytest.raises(ValueError):
+        m.broadcast_density_to_mask(np.zeros(K, np.uint8), lab)
+
+
 def test_connectivity_table_overflow_falls_back_to_the_scan(checker):
     """A label map with far more distinct adjacent pairs than a superpixel map has: the pair table overflows and the
     single-thread replay of the reference's loop takes over (exact, slow)."""
