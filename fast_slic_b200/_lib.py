@@ -35,6 +35,8 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_crfdev_push_scratch_bytes", "fslic_b200_crfdev_push_label_frames", "fslic_b200_crfdev_set_unary",
     "fslic_b200_crfdev_set_proba", "fslic_b200_crfdev_set_mask", "fslic_b200_crfdev_get_inferred",
     "fslic_b200_debug_logf_host", "fslic_b200_debug_logf_device",
+    "fslic_b200_crfgroup_inference", "fslic_b200_crfdev_group_push_label_frames", "fslic_b200_crfdev_group_set_proba",
+    "fslic_b200_crfdev_group_reset_inferred", "fslic_b200_crfdev_group_get_inferred", "fslic_b200_crfgroup_pop_frame",
 )
 
 STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity", "iterate")

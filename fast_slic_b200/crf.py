@@ -25,10 +25,26 @@ labels and uint8 [K,32] cluster records that `iterate_batch(..., return_clusters
 That work is enqueued on the CRF device's current torch stream, and every frame equals what the host path stores for
 the same values, bit for bit.
 
+`SimpleCRFGroup` drives the CRFs of many video streams together, one SimpleCRF per stream with the same num_classes,
+num_nodes and device, in the same kernel launches: image b of each batch is the next frame of member b::
+
+    crfs = [SimpleCRF(C, K) for _ in range(B)]
+    group = SimpleCRFGroup(crfs)
+    labels, clusters = slic.iterate_batch(images, return_clusters=True)   # [B,H,W], [B,K,32]
+    group.push_label_frames(labels, clusters)                             # one frame per member
+    group.set_proba(proba); group.reset_inferred()                        # float32 cuda [B, C, K]
+    group.inference(5)
+    group.get_inferred(out=q)                                             # float32 cuda [B, C, K]
+    group.pop_frame()
+
+Every member computes exactly what its own calls compute, and keeps its whole surface (frames, host getters,
+energies, its own inference).
+
 Where the reference reads out of bounds or crashes, this module raises instead: neighbour
 indices or mask classes outside the frame raise ValueError and change nothing, and a frame handle whose frame was
 popped raises IndexError.
 """
+import contextlib
 import ctypes as C
 import operator
 import threading
@@ -39,7 +55,7 @@ import torch
 from . import _lib
 from .engine import CLUSTER_DTYPE
 
-__all__ = ["SimpleCRF", "SimpleCRFFrame"]
+__all__ = ["SimpleCRF", "SimpleCRFFrame", "SimpleCRFGroup"]
 
 _PARAM_NAMES = ("spatial_w", "temporal_w", "spatial_srgb", "temporal_srgb", "spatial_sxy", "spatial_smooth_w",
                 "spatial_smooth_sxy")
@@ -87,6 +103,12 @@ def _L():
         for name in ("set_unary", "set_proba", "get_inferred"):
             getattr(L, "fslic_b200_crfdev_" + name).argtypes = [vp, i32, vp, vp]
         L.fslic_b200_crfdev_set_mask.argtypes = [vp, i32, vp, C.c_float, vp]
+        L.fslic_b200_crfgroup_inference.argtypes = [vp, i32, C.c_ulonglong, vp]
+        L.fslic_b200_crfdev_group_push_label_frames.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, C.c_size_t, vp, ip]
+        for name in ("set_proba", "get_inferred"):
+            getattr(L, "fslic_b200_crfdev_group_" + name).argtypes = [vp, i32, vp, vp]
+        L.fslic_b200_crfdev_group_reset_inferred.argtypes = [vp, i32, vp]
+        L.fslic_b200_crfgroup_pop_frame.argtypes = [vp, i32, ip]
         _bound = True
     return L
 
@@ -505,3 +527,123 @@ class SimpleCRF(object):
         max_iter = _size_t(max_iter)
         with self.lock:
             _check(_L().fslic_b200_crf_inference(self._h, max_iter, None))
+
+
+class SimpleCRFGroup(object):
+    """The SimpleCRFs `crfs` (distinct, with the same num_classes, num_nodes and device) driven together: each call
+    runs every member in the same kernel launches, on the device's current torch stream, and leaves every member as
+    its own calls would.  Member b takes image b of each batch.  The members keep their whole surface; the group holds
+    no state of its own besides the list."""
+
+    def __init__(self, crfs):
+        crfs = list(crfs)
+        if not crfs:
+            raise ValueError("a SimpleCRFGroup needs at least one SimpleCRF")
+        if not all(isinstance(c, SimpleCRF) for c in crfs):
+            raise ValueError("every member must be a SimpleCRF")
+        if len(set(map(id, crfs))) != len(crfs):
+            raise ValueError("a SimpleCRF is in the group twice")
+        c0 = crfs[0]
+        if any((c._C, c._N, c.device) != (c0._C, c0._N, c0.device) for c in crfs):
+            raise ValueError("members differ in num_classes, num_nodes or device")
+        self._crfs = crfs
+        self._handles = (C.c_void_p * len(crfs))(*[c._h.value for c in crfs])
+        self._locks = [c.lock for c in sorted(crfs, key=id)]  # one global order, as temporal_pairwise_energy takes it
+
+    def _stream(self):
+        return self._crfs[0]._stream()
+
+    @property
+    def crfs(self):
+        return list(self._crfs)
+
+    def __len__(self):
+        return len(self._crfs)
+
+    @contextlib.contextmanager
+    def _locked(self):
+        """The members' device current and all their locks held."""
+        with contextlib.ExitStack() as stack:
+            stack.enter_context(torch.cuda.device(torch.device("cuda", self._crfs[0].device)))
+            for lock in self._locks:
+                stack.enter_context(lock)
+            yield
+
+    def _call(self, name, *args, first=0, count=None):
+        """fslic_b200_<name> over members first .. first + count - 1 (default: all), under _locked()."""
+        n = len(self._crfs) - first if count is None else count
+        handles = C.c_void_p(C.addressof(self._handles) + first * C.sizeof(C.c_void_p))
+        with self._locked():
+            _check(getattr(_L(), "fslic_b200_" + name)(handles, n, *args))
+
+    def _group_tensor(self, x, cname="float"):
+        c0 = self._crfs[0]
+        _device_tensor(x, c0.device, torch.float32, 3, cname)
+        want = (len(self._crfs), c0._C, c0._N)
+        if tuple(x.shape) != want:
+            raise ValueError("expected a tensor of shape %s, got %s" % (want, tuple(x.shape)))
+        return x
+
+    def push_label_frames(self, labels, clusters):
+        """Frame b from int16 cuda labels[b] ([B,H,W]) and uint8 cuda records clusters[b] ([B,K,32]), B = len(group),
+        appended to member b: what member b's own push_label_frames(labels[b], clusters[b]) gives.  Every argument is
+        checked (ValueError) before anything is pushed.  Returns the new SimpleCRFFrame of each member."""
+        from .graph_batch import graph_chunk
+        if not _is_cuda(labels) or not _is_cuda(clusters):
+            raise ValueError("labels and clusters must be cuda tensors")
+        c0 = self._crfs[0]
+        B, K = len(self._crfs), c0._N
+        _device_tensor(labels, c0.device, torch.int16, 3, "int16_t")
+        _device_tensor(clusters, c0.device, torch.uint8, 3, "uint8_t")
+        if labels.shape[0] != B or tuple(clusters.shape) != (B, K, 32):
+            raise ValueError("labels must be [%d,H,W] and clusters [%d,%d,32], got %s and %s" % (
+                B, B, K, tuple(labels.shape), tuple(clusters.shape)))
+        H, W = int(labels.shape[1]), int(labels.shape[2])
+        if H == 0 or W == 0:
+            raise ValueError("labels must have at least one pixel")
+        if not 1 <= K <= 65535:
+            raise ValueError("push_label_frames needs 1 <= num_nodes <= 65535, the range of the labels")
+        lab, cl = labels.contiguous(), clusters.contiguous()
+        times = np.zeros(B, np.int32)
+        with self._locked():
+            chunk = graph_chunk(K, B)  # images whose graph scratch stays under GRAPH_SCRATCH_CAP
+            nbytes = int(_L().fslic_b200_crfdev_push_scratch_bytes(K, chunk))
+            scratch = torch.empty(nbytes, dtype=torch.uint8, device=torch.device("cuda", c0.device))
+            for b0 in range(0, B, chunk):
+                self._call("crfdev_group_push_label_frames", H, W, K, lab[b0].data_ptr(), cl[b0].data_ptr(),
+                           scratch.data_ptr(), nbytes, c0._stream(), times[b0:].ctypes.data_as(C.POINTER(C.c_int)),
+                           first=b0, count=min(chunk, B - b0))
+        return [SimpleCRFFrame(c, int(t)) for c, t in zip(self._crfs, times)]
+
+    def set_proba(self, proba):
+        """set_proba of each member's newest frame from float32 cuda proba [B, C, N] (-logf(p))."""
+        self._call("crfdev_group_set_proba", self._group_tensor(proba).contiguous().data_ptr(), self._stream())
+
+    def reset_inferred(self):
+        """reset_inferred of each member's newest frame."""
+        self._call("crfdev_group_reset_inferred", self._stream())
+
+    def inference(self, max_iter):
+        """max_iter mean-field steps of every member, asynchronously."""
+        self._call("crfgroup_inference", _size_t(max_iter), self._stream())
+
+    def get_inferred(self, out=None):
+        """q of each member's newest frame into the contiguous float32 cuda tensor `out` [B, C, N] (a new one if None),
+        enqueued on the current stream; returns it."""
+        c0 = self._crfs[0]
+        if out is None:
+            out = torch.empty((len(self._crfs), c0._C, c0._N), dtype=torch.float32,
+                              device=torch.device("cuda", c0.device))
+        if not _is_cuda(out):
+            raise ValueError("out must be a cuda float32 tensor of shape [len(group), num_classes, num_nodes]")
+        self._group_tensor(out)
+        if not out.is_contiguous():
+            raise ValueError("out must be contiguous")
+        self._call("crfdev_group_get_inferred", out.data_ptr(), self._stream())
+        return out
+
+    def pop_frame(self):
+        """pop_frame of every member; the popped times, -1 for a member that had no frames."""
+        times = np.zeros(len(self._crfs), np.int32)
+        self._call("crfgroup_pop_frame", times.ctypes.data_as(C.POINTER(C.c_int)))
+        return times.tolist()

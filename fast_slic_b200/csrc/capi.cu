@@ -6,10 +6,12 @@
 #include <limits.h>
 #include <math.h>
 #include <stdlib.h>
+#include <algorithm>
 #include <new>
 #include <cstring>
 #include <deque>
 #include <string>
+#include <unordered_set>
 #include <vector>
 
 #include "assign.cuh"
@@ -2026,7 +2028,9 @@ static int crf_take_slot(fslic_crf* c, CrfSlot** out) {
                            std::string(#call) + ": " + cudaGetErrorString(e__));                      \
     } while (0)
 
-static int crf_upload_table(fslic_crf* c) {
+// Enqueues the upload of the frame table on the CRF's stream from `h`, which must live until that stream is
+// synchronised.
+static int crf_stage_table(fslic_crf* c, std::vector<CrfFrameDev>& h) {
     const size_t T = c->frames.size();
     if (T > c->table_cap) {
         cudaFree(c->d_table);
@@ -2035,12 +2039,19 @@ static int crf_upload_table(fslic_crf* c) {
         CKA(cudaMalloc(&c->d_table, sizeof(CrfFrameDev) * T * 2));
         c->table_cap = T * 2;
     }
-    std::vector<CrfFrameDev> h(T);
+    h.resize(T);
     for (size_t t = 0; t < T; t++) {
         const CrfSlot* s = c->frames[t];
         h[t] = CrfFrameDev{s->clusters, s->offsets, s->nbr, s->unary, {s->q0, s->q1}, s->msg, s->e_sp, s->r_sp, s->tmp};
     }
     if (T) CK(cudaMemcpyAsync(c->d_table, h.data(), sizeof(CrfFrameDev) * T, cudaMemcpyHostToDevice, c->st));
+    return FSLIC_OK;
+}
+
+static int crf_upload_table(fslic_crf* c) {
+    std::vector<CrfFrameDev> h;
+    int rc = crf_stage_table(c, h);
+    if (rc) return rc;
     CK(cudaStreamSynchronize(c->st));
     return FSLIC_OK;
 }
@@ -2340,12 +2351,21 @@ extern "C" int fslic_b200_crf_get_inferred(fslic_crf* c, int time, float* h_out)
     return FSLIC_OK;
 }
 
-static int crf_reset(fslic_crf* c, CrfSlot* s) {
-    const long long CN = (long long)c->C * c->N;
-    if (!CN) return FSLIC_OK;
-    k_crf_reset<<<(unsigned)((CN + 255) / 256), 256, 0, c->st>>>(s->unary, c->cur ? s->q1 : s->q0, CN);
+// The unaries and current q buffer of a frame, for the per-frame kernels
+static CrfFrameQ crf_frame_q(const fslic_crf* c, const CrfSlot* s) { return CrfFrameQ{s->unary, c->cur ? s->q1 : s->q0}; }
+
+// reset_inferred of the frames of `set` (n <= CRF_GROUP_MAX, C * N values each) in one launch
+static int crf_reset_set(const CrfFrameQSet& set, int n, long long CN, int device, cudaStream_t st) {
+    if (!CN || !n) return FSLIC_OK;
+    k_crf_reset<<<dim3((unsigned)grid_for(CN, device), (unsigned)n), 256, 0, st>>>(set, CN);
     CK(cudaGetLastError());
     return FSLIC_OK;
+}
+
+static int crf_reset(fslic_crf* c, CrfSlot* s) {
+    CrfFrameQSet set;
+    set.f[0] = crf_frame_q(c, s);
+    return crf_reset_set(set, 1, (long long)c->C * c->N, c->device, c->st);
 }
 
 // SimpleCRFFrame::reset_inferred (simple-crf.cpp:57-59): q = expf(-unary), asynchronous on the CRF's stream
@@ -2361,10 +2381,40 @@ extern "C" int fslic_b200_crf_reset_inferred(fslic_crf* c, int time) {
 extern "C" int fslic_b200_crf_initialize(fslic_crf* c) {
     if (!c) return set_err(FSLIC_EINVAL, "crf is NULL");
     USE_DEVICE(c->device);
-    for (CrfSlot* s : c->frames) {
-        int rc = crf_reset(c, s);
+    const long long CN = (long long)c->C * c->N;
+    for (size_t t0 = 0; t0 < c->frames.size(); t0 += CRF_GROUP_MAX) {
+        const int n = (int)std::min(c->frames.size() - t0, (size_t)CRF_GROUP_MAX);
+        CrfFrameQSet set;
+        for (int k = 0; k < n; k++) set.f[k] = crf_frame_q(c, c->frames[t0 + k]);
+        int rc = crf_reset_set(set, n, CN, c->device, c->st);
         if (rc) return rc;
     }
+    return FSLIC_OK;
+}
+
+// max_iter Jacobi steps of the chains of crfs[0 .. n) (n <= CRF_GROUP_MAX; one device, C and N; each with frames) on
+// `st`: 1 + 2 max_iter launches; each CRF's cur flips once per step.  With N or C zero there is nothing to compute and
+// cur stays.
+static int crf_run_chains(fslic_crf* const* crfs, int n, unsigned long long max_iter, cudaStream_t st) {
+    const int C = crfs[0]->C, N = crfs[0]->N;
+    if (!n || !max_iter || !N || !C) return FSLIC_OK;
+    CrfChainSet set;
+    long long Tmax = 0;
+    for (int k = 0; k < n; k++) {
+        const fslic_crf* c = crfs[k];
+        set.ch[k] = CrfChain{c->d_table, (int)c->frames.size(), c->cur, c->p};
+        Tmax = std::max(Tmax, (long long)c->frames.size());
+    }
+    const long long TN = Tmax * N, TCN = TN * C;
+    const dim3 node_grid((unsigned)((TN + 127) / 128), (unsigned)n), msg_grid((unsigned)((TCN + 127) / 128), (unsigned)n);
+    k_crf_pairwise<<<node_grid, 128, 0, st>>>(set, N);
+    CK(cudaGetLastError());
+    for (unsigned long long it = 0; it < max_iter; it++) {
+        k_crf_msg<<<msg_grid, 128, 0, st>>>(set, N, C, (int)(it & 1));
+        k_crf_compat<<<node_grid, 128, 0, st>>>(set, N, C, (int)(it & 1));
+        CK(cudaGetLastError());
+    }
+    for (int k = 0; k < n; k++) crfs[k]->cur ^= (int)(max_iter & 1);
     return FSLIC_OK;
 }
 
@@ -2380,20 +2430,7 @@ extern "C" int fslic_b200_crf_inference(fslic_crf* c, unsigned long long max_ite
         CK(cudaStreamSynchronize(c->st));
         c->st = (cudaStream_t)stream;
     }
-    const long long TN = (long long)c->frames.size() * c->N;
-    if (!TN || !c->C) return FSLIC_OK;
-    const int T = (int)c->frames.size();
-    const unsigned blocks = (unsigned)((TN + 127) / 128);
-    k_crf_pairwise<<<blocks, 128, 0, c->st>>>(c->d_table, T, c->N, c->p);
-    CK(cudaGetLastError());
-    const long long TCN = TN * c->C;
-    for (unsigned long long it = 0; it < max_iter; it++) {
-        k_crf_msg<<<(unsigned)((TCN + 127) / 128), 128, 0, c->st>>>(c->d_table, T, c->N, c->C, c->cur);
-        k_crf_compat<<<blocks, 128, 0, c->st>>>(c->d_table, T, c->N, c->C, c->cur);
-        CK(cudaGetLastError());
-        c->cur ^= 1;
-    }
-    return FSLIC_OK;
+    return crf_run_chains(&c, 1, max_iter, c->st);
 }
 
 // SimpleCRFFrame::calc_spatial_pairwise_energy(node_i, node_j) of frame `time` (simple-crf.hpp:149-174)
@@ -2517,6 +2554,91 @@ static int crfdev_take_slot(fslic_crf* c, CrfSlot** out) {
     return FSLIC_OK;
 }
 
+// The argument checks of a device push of `batch` label maps into CRFs with N == K nodes.
+static int crfdev_check_push(int batch, int H, int W, int K, const uint16_t* d_labels, const fslic_cluster* d_clusters,
+                             void* d_scratch, size_t scratch_bytes) {
+    if (batch < 0 || H <= 0 || W <= 0 || K <= 0 || K > 65535) return set_err(FSLIC_EINVAL, "bad batch, H, W or K");
+    if (batch == 0) return FSLIC_OK;
+    if (!d_labels || !d_clusters || !d_scratch) return set_err(FSLIC_EINVAL, "NULL argument");
+    const size_t need = fslic_b200_crfdev_push_scratch_bytes(K, batch);
+    if (need == (size_t)-1) return set_err(FSLIC_EINVAL, "batch too large for one call");
+    if (scratch_bytes < need) return set_err(FSLIC_EINVAL, "scratch too small");
+    const int obits = bit_length(3ull * (unsigned long long)H * (unsigned long long)W);
+    if (obits + bit_length(batch - 1) > 64) return set_err(FSLIC_EINVAL, "batch * H * W too large");
+    return FSLIC_OK;
+}
+
+// Appends frame b, built from d_labels[b] and d_clusters[b], to owners[b] (all on one device with the same C and
+// N == K, all already on `stream`; a CRF may own several frames, which it receives in order).  Arguments are checked
+// by the caller.  The new frames join their tables first, so the one host wait (after the table uploads) does not
+// include this push's kernels.  On failure every owner is left as it was.
+static int crfdev_push(fslic_crf* const* owners, int batch, int H, int W, int K, const uint16_t* d_labels,
+                       const fslic_cluster* d_clusters, void* d_scratch, cudaStream_t st, int* times_out) {
+    std::vector<CrfSlot*> slots;
+    for (int b = 0; b < batch; b++) {
+        CrfSlot* s = nullptr;
+        int rc = crfdev_take_slot(owners[b], &s);
+        if (rc) {
+            for (int k = 0; k < b; k++) owners[k]->pool.push_back(slots[k]);
+            return rc;
+        }
+        slots.push_back(s);
+    }
+    std::vector<fslic_crf*> distinct;
+    for (int b = 0; b < batch; b++) {
+        fslic_crf* c = owners[b];
+        if (std::find(distinct.begin(), distinct.end(), c) == distinct.end()) distinct.push_back(c);
+        slots[b]->time = c->next_time++;
+        c->frames.push_back(slots[b]);
+    }
+    int rc = FSLIC_OK;
+    {
+        std::vector<std::vector<CrfFrameDev>> tables(distinct.size());
+        for (size_t k = 0; k < distinct.size() && !rc; k++) rc = crf_stage_table(distinct[k], tables[k]);
+        const cudaError_t e = cudaStreamSynchronize(st);
+        if (!rc && e != cudaSuccess) rc = set_err(FSLIC_ECUDA, std::string("cudaStreamSynchronize: ") + cudaGetErrorString(e));
+    }
+    const fslic_crf* c0 = owners[0];
+    if (!rc) {
+        const size_t graph_bytes = align_up(fslic_b200_connectivity_batch_scratch_bytes(K, batch), 256);
+        unsigned char* p = static_cast<unsigned char*>(d_scratch);
+        int32_t* counts = reinterpret_cast<int32_t*>(p + graph_bytes);
+        uint32_t* nbrs = reinterpret_cast<uint32_t*>(p + graph_bytes + align_up((size_t)batch * K * 4, 256));
+        rc = fslic_b200_get_connectivity_batch(c0->device, batch, H, W, K, d_labels, counts, nbrs, nullptr, d_scratch,
+                                               graph_bytes, st);
+        const long long CN = (long long)c0->C * K;
+        const float unbiased = logf((float)c0->C);  // set_unbiased's constant, glibc's logf as on the host path
+        const unsigned node_blocks = (unsigned)grid_for(CN > K ? CN : K, c0->device);
+        for (int b0 = 0; b0 < batch && !rc; b0 += CRF_GROUP_MAX) {
+            const int n = std::min(batch - b0, CRF_GROUP_MAX);
+            FeedFrameSet dst;
+            for (int k = 0; k < n; k++) {
+                const CrfSlot* s = slots[b0 + k];
+                dst.f[k] = FeedFramePtrs{s->clusters, s->unary, s->q0, s->q1, s->offsets, s->nbr};
+            }
+            k_feed_nodes<<<dim3(node_blocks, (unsigned)n), 256, 0, st>>>(d_clusters + (size_t)b0 * K, dst, K, c0->C,
+                                                                         unbiased);
+            k_feed_csr<<<dim3(1, (unsigned)n), FEED_CSR_THREADS, 0, st>>>(counts + (size_t)b0 * K,
+                                                                          nbrs + (size_t)b0 * K * CONN_MAX, K, dst);
+            const cudaError_t e = cudaGetLastError();
+            if (e != cudaSuccess) rc = set_err(FSLIC_ECUDA, std::string("feed kernels: ") + cudaGetErrorString(e));
+        }
+    }
+    if (rc) {  // take the frames back out, newest first
+        for (int b = batch - 1; b >= 0; b--) {
+            fslic_crf* c = owners[b];
+            c->pool.push_back(c->frames.back());
+            c->frames.pop_back();
+            c->next_time--;
+        }
+        for (fslic_crf* c : distinct) crf_upload_table(c);
+        return rc;
+    }
+    if (times_out)
+        for (int b = 0; b < batch; b++) times_out[b] = slots[b]->time;
+    return FSLIC_OK;
+}
+
 // Pushes `batch` frames; frame b is what push_slic_frame gives for label map d_labels[b] (int16 [H][W], labels outside
 // [0, K) ignored) and records d_clusters[b] ([K]): its records, its adjacency graph and unbiased unaries.  K must equal
 // the CRF's num_nodes.  Every argument is checked before anything is pushed (the host push_slic_frame pushes a blank
@@ -2526,64 +2648,12 @@ extern "C" int fslic_b200_crfdev_push_label_frames(fslic_crf* c, int batch, int 
                                                    void* stream, int* times_out) {
     if (!c) return set_err(FSLIC_EINVAL, "crf is NULL");
     if (K != c->N) return set_err(FSLIC_EINVAL, "K must equal the CRF's num_nodes");
-    if (batch < 0 || H <= 0 || W <= 0 || K <= 0 || K > 65535) return set_err(FSLIC_EINVAL, "bad batch, H, W or K");
+    { int rc = crfdev_check_push(batch, H, W, K, d_labels, d_clusters, d_scratch, scratch_bytes); if (rc) return rc; }
     if (batch == 0) return FSLIC_OK;
-    if (!d_labels || !d_clusters || !d_scratch) return set_err(FSLIC_EINVAL, "NULL argument");
-    const size_t need = fslic_b200_crfdev_push_scratch_bytes(K, batch);
-    if (need == (size_t)-1) return set_err(FSLIC_EINVAL, "batch too large for one call");
-    if (scratch_bytes < need) return set_err(FSLIC_EINVAL, "scratch too small");
-    const int obits = bit_length(3ull * (unsigned long long)H * (unsigned long long)W);
-    if (obits + bit_length(batch - 1) > 64) return set_err(FSLIC_EINVAL, "batch * H * W too large");
     USE_DEVICE(c->device);
     { int rc = crf_adopt_stream(c, stream); if (rc) return rc; }
-    std::vector<CrfSlot*> slots;
-    for (int b = 0; b < batch; b++) {
-        CrfSlot* s = nullptr;
-        int rc = crfdev_take_slot(c, &s);
-        if (rc) {
-            for (CrfSlot* t : slots) c->pool.push_back(t);
-            return rc;
-        }
-        slots.push_back(s);
-    }
-    // the new frames join the table first, so the one host wait (the table upload) does not include this push's work
-    const int next_time0 = c->next_time;
-    for (CrfSlot* s : slots) {
-        s->time = c->next_time++;
-        c->frames.push_back(s);
-    }
-    int rc = crf_upload_table(c);
-    if (!rc) {
-        const size_t graph_bytes = align_up(fslic_b200_connectivity_batch_scratch_bytes(K, batch), 256);
-        unsigned char* p = static_cast<unsigned char*>(d_scratch);
-        int32_t* counts = reinterpret_cast<int32_t*>(p + graph_bytes);
-        uint32_t* nbrs = reinterpret_cast<uint32_t*>(p + graph_bytes + align_up((size_t)batch * K * 4, 256));
-        rc = fslic_b200_get_connectivity_batch(c->device, batch, H, W, K, d_labels, counts, nbrs, nullptr, d_scratch,
-                                               graph_bytes, stream);
-        const long long CN = (long long)c->C * K;
-        const float unbiased = logf((float)c->C);  // set_unbiased's constant, glibc's logf as on the host path
-        for (int b = 0; b < batch && !rc; b++) {
-            CrfSlot* s = slots[b];
-            k_feed_nodes<<<(int)grid_for(CN > K ? CN : K, c->device), 256, 0, c->st>>>(
-                d_clusters + (size_t)b * K, FeedFramePtrs{s->clusters, s->unary, s->q0, s->q1}, K, c->C, unbiased);
-            k_feed_csr<<<1, FEED_CSR_THREADS, 0, c->st>>>(counts + (size_t)b * K, nbrs + (size_t)b * K * CONN_MAX, K,
-                                                          s->offsets, s->nbr);
-            const cudaError_t e = cudaGetLastError();
-            if (e != cudaSuccess) rc = set_err(FSLIC_ECUDA, std::string("feed kernels: ") + cudaGetErrorString(e));
-        }
-    }
-    if (rc) {  // take the frames back out
-        for (int b = 0; b < batch; b++) {
-            c->pool.push_back(c->frames.back());
-            c->frames.pop_back();
-        }
-        c->next_time = next_time0;
-        crf_upload_table(c);
-        return rc;
-    }
-    if (times_out)
-        for (int b = 0; b < batch; b++) times_out[b] = slots[b]->time;
-    return FSLIC_OK;
+    const std::vector<fslic_crf*> owners(batch, c);
+    return crfdev_push(owners.data(), batch, H, W, K, d_labels, d_clusters, d_scratch, c->st, times_out);
 }
 
 // Look up frame `time`, switch to the CRF's device and adopt `stream`: the device setters never wait for it.
@@ -2608,7 +2678,9 @@ extern "C" int fslic_b200_crfdev_set_proba(fslic_crf* c, int time, const float* 
     const long long CN = (long long)c->C * c->N;
     if (!CN) return FSLIC_OK;
     if (!d_proba) return set_err(FSLIC_EINVAL, "NULL argument");
-    k_feed_proba<<<(int)grid_for(CN, c->device), 256, 0, c->st>>>(d_proba, s->unary, CN);
+    CrfFrameQSet set;
+    set.f[0] = crf_frame_q(c, s);
+    k_feed_proba<<<(unsigned)grid_for(CN, c->device), 256, 0, c->st>>>(d_proba, set, CN);
     CK(cudaGetLastError());
     return FSLIC_OK;
 }
@@ -2646,6 +2718,151 @@ extern "C" int fslic_b200_crfdev_get_inferred(fslic_crf* c, int time, float* d_o
     if (CN && !d_out) return set_err(FSLIC_EINVAL, "NULL argument");
     if (CN) CK(cudaMemcpyAsync(d_out, c->cur ? s->q1 : s->q0, sizeof(float) * CN, cudaMemcpyDeviceToDevice, c->st));
     return FSLIC_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Groups: crfs[0 .. n) are distinct CRFs on one device with the same C and N, typically one per video stream, driven
+// in the same launches (CRF_GROUP_MAX members per launch set).  Every call checks all members before it enqueues
+// anything, so a refused call changes none of them; it adopts `stream` for every member like crf_adopt_stream, with one
+// wait per different stream the members were on; and it leaves each member in the state (cur, stream, frame table,
+// stale host copies) its own entry points would have left it in.
+
+static int crf_group_check(fslic_crf* const* crfs, int n, bool need_frames) {
+    if (n < 0 || (n && !crfs)) return set_err(FSLIC_EINVAL, "bad group");
+    std::unordered_set<const fslic_crf*> seen;
+    for (int k = 0; k < n; k++) {
+        const fslic_crf* c = crfs[k];
+        if (!c) return set_err(FSLIC_EINVAL, "crf is NULL");
+        if (!seen.insert(c).second) return set_err(FSLIC_EINVAL, "a CRF is in the group twice");
+        if (c->device != crfs[0]->device || c->C != crfs[0]->C || c->N != crfs[0]->N)
+            return set_err(FSLIC_EINVAL, "group members differ in device, num_classes or num_nodes");
+    }
+    if (need_frames)
+        for (int k = 0; k < n; k++)
+            if (crfs[k]->frames.empty()) return set_err(FSLIC_ENOFRAME, "Time out of range");
+    return FSLIC_OK;
+}
+
+static int crf_group_adopt(fslic_crf* const* crfs, int n, void* stream) {
+    std::vector<cudaStream_t> waited;
+    for (int k = 0; k < n; k++) {
+        fslic_crf* c = crfs[k];
+        if (c->st == (cudaStream_t)stream) continue;
+        if (std::find(waited.begin(), waited.end(), c->st) == waited.end()) {
+            CK(cudaStreamSynchronize(c->st));
+            waited.push_back(c->st);
+        }
+        c->st = (cudaStream_t)stream;
+    }
+    return FSLIC_OK;
+}
+
+// The newest frame of each of crfs[0 .. n), n <= CRF_GROUP_MAX
+static CrfFrameQSet crf_group_newest(fslic_crf* const* crfs, int n) {
+    CrfFrameQSet set;
+    for (int k = 0; k < n; k++) set.f[k] = crf_frame_q(crfs[k], crfs[k]->frames.back());
+    return set;
+}
+
+extern "C" int fslic_b200_crfgroup_inference(fslic_crf* const* crfs, int n, unsigned long long max_iter, void* stream) {
+    { int rc = crf_group_check(crfs, n, max_iter > 0); if (rc) return rc; }
+    if (!n || !max_iter) return FSLIC_OK;
+    USE_DEVICE(crfs[0]->device);
+    { int rc = crf_group_adopt(crfs, n, stream); if (rc) return rc; }
+    for (int k0 = 0; k0 < n; k0 += CRF_GROUP_MAX) {
+        int rc = crf_run_chains(crfs + k0, std::min(n - k0, CRF_GROUP_MAX), max_iter, (cudaStream_t)stream);
+        if (rc) return rc;
+    }
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_crfdev_group_push_label_frames(fslic_crf* const* crfs, int n, int H, int W, int K,
+                                                         const uint16_t* d_labels, const fslic_cluster* d_clusters,
+                                                         void* d_scratch, size_t scratch_bytes, void* stream,
+                                                         int* times_out) {
+    { int rc = crf_group_check(crfs, n, false); if (rc) return rc; }
+    if (n && K != crfs[0]->N) return set_err(FSLIC_EINVAL, "K must equal the CRFs' num_nodes");
+    { int rc = crfdev_check_push(n, H, W, K, d_labels, d_clusters, d_scratch, scratch_bytes); if (rc) return rc; }
+    if (!n) return FSLIC_OK;
+    USE_DEVICE(crfs[0]->device);
+    { int rc = crf_group_adopt(crfs, n, stream); if (rc) return rc; }
+    return crfdev_push(crfs, n, H, W, K, d_labels, d_clusters, d_scratch, (cudaStream_t)stream, times_out);
+}
+
+extern "C" int fslic_b200_crfdev_group_set_proba(fslic_crf* const* crfs, int n, const float* d_proba, void* stream) {
+    { int rc = crf_group_check(crfs, n, true); if (rc) return rc; }
+    if (!n) return FSLIC_OK;
+    const long long CN = (long long)crfs[0]->C * crfs[0]->N;
+    if (CN && !d_proba) return set_err(FSLIC_EINVAL, "NULL argument");
+    const int device = crfs[0]->device;
+    USE_DEVICE(device);
+    { int rc = crf_group_adopt(crfs, n, stream); if (rc) return rc; }
+    if (!CN) return FSLIC_OK;
+    for (int k0 = 0; k0 < n; k0 += CRF_GROUP_MAX) {
+        const int m = std::min(n - k0, CRF_GROUP_MAX);
+        k_feed_proba<<<dim3((unsigned)grid_for(CN, device), (unsigned)m), 256, 0, (cudaStream_t)stream>>>(
+            d_proba + (size_t)k0 * CN, crf_group_newest(crfs + k0, m), CN);
+        CK(cudaGetLastError());
+    }
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_crfdev_group_reset_inferred(fslic_crf* const* crfs, int n, void* stream) {
+    { int rc = crf_group_check(crfs, n, true); if (rc) return rc; }
+    if (!n) return FSLIC_OK;
+    const int device = crfs[0]->device;
+    USE_DEVICE(device);
+    { int rc = crf_group_adopt(crfs, n, stream); if (rc) return rc; }
+    const long long CN = (long long)crfs[0]->C * crfs[0]->N;
+    for (int k0 = 0; k0 < n; k0 += CRF_GROUP_MAX) {
+        const int m = std::min(n - k0, CRF_GROUP_MAX);
+        int rc = crf_reset_set(crf_group_newest(crfs + k0, m), m, CN, device, (cudaStream_t)stream);
+        if (rc) return rc;
+    }
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_crfdev_group_get_inferred(fslic_crf* const* crfs, int n, float* d_out, void* stream) {
+    { int rc = crf_group_check(crfs, n, true); if (rc) return rc; }
+    if (!n) return FSLIC_OK;
+    const long long CN = (long long)crfs[0]->C * crfs[0]->N;
+    if (CN && !d_out) return set_err(FSLIC_EINVAL, "NULL argument");
+    const int device = crfs[0]->device;
+    USE_DEVICE(device);
+    { int rc = crf_group_adopt(crfs, n, stream); if (rc) return rc; }
+    if (!CN) return FSLIC_OK;
+    for (int k0 = 0; k0 < n; k0 += CRF_GROUP_MAX) {
+        const int m = std::min(n - k0, CRF_GROUP_MAX);
+        k_crf_get_q<<<dim3((unsigned)grid_for(CN, device), (unsigned)m), 256, 0, (cudaStream_t)stream>>>(
+            crf_group_newest(crfs + k0, m), d_out + (size_t)k0 * CN, CN);
+        CK(cudaGetLastError());
+    }
+    return FSLIC_OK;
+}
+
+// pop_frame of every member: the table uploads of all of them, then one wait per stream the members are on.
+extern "C" int fslic_b200_crfgroup_pop_frame(fslic_crf* const* crfs, int n, int* times_out) {
+    { int rc = crf_group_check(crfs, n, false); if (rc) return rc; }
+    if (!n) return FSLIC_OK;
+    USE_DEVICE(crfs[0]->device);
+    std::vector<std::vector<CrfFrameDev>> tables(n);
+    std::vector<cudaStream_t> streams;
+    int rc = FSLIC_OK;
+    for (int k = 0; k < n; k++) {
+        fslic_crf* c = crfs[k];
+        if (c->frames.empty()) {
+            if (times_out) times_out[k] = -1;
+            continue;
+        }
+        CrfSlot* s = c->frames.front();
+        c->frames.pop_front();
+        c->pool.push_back(s);
+        if (times_out) times_out[k] = s->time;
+        if (!rc) rc = crf_stage_table(c, tables[k]);
+        if (std::find(streams.begin(), streams.end(), c->st) == streams.end()) streams.push_back(c->st);
+    }
+    for (cudaStream_t st : streams) CK(cudaStreamSynchronize(st));
+    return rc;
 }
 
 extern "C" int fslic_b200_debug_logf_host(uint32_t first, long long n, float* h_out) {

@@ -6,6 +6,7 @@
 #include <cub/block/block_scan.cuh>
 #include "common.cuh"
 #include "glibc_logf.cuh"
+#include "crf.cuh"
 
 // numpy's float64 -> int32 cast on x86 (cvttsd2si): truncation, and INT_MIN for NaN, ±inf and anything whose truncation
 // is outside the int32 range.  CUDA's conversion saturates and maps NaN to 0, so those cases are spelled out.
@@ -17,15 +18,23 @@ __device__ __forceinline__ int32_t feed_x86_trunc_i32(double d) {
 // (round to nearest) and num_members as uint32 (wrapping), `number` = index as uint16, every other field zero.
 __device__ __forceinline__ float feed_coord(float v) { return __int2float_rn(feed_x86_trunc_i32((double)v)); }
 
-// One thread per node of each frame of a batch: records of frame b go to dst[b].  Also fills the frame's unaries with
-// `unbiased` (set_unbiased: logf(C), the host's constant) and zeroes both q buffers, as push_frame does.
+// The destinations of up to CRF_GROUP_MAX pushed frames (crf.cuh), blockIdx.y = frame of the launch.
 struct FeedFramePtrs {
     fslic_cluster* clusters;
     float *unary, *q0, *q1;
+    int32_t *offsets, *nbr;
+};
+struct FeedFrameSet {
+    FeedFramePtrs f[CRF_GROUP_MAX];
 };
 
-__global__ void __launch_bounds__(256) k_feed_nodes(const fslic_cluster* __restrict__ src, FeedFramePtrs dst, int N, int C,
+// One thread per node of each frame: records src[blockIdx.y] ([N]) go to frame blockIdx.y.  Also fills the frame's
+// unaries with `unbiased` (set_unbiased: logf(C), the host's constant) and zeroes both q buffers, as push_frame does.
+__global__ void __launch_bounds__(256) k_feed_nodes(const fslic_cluster* __restrict__ src,
+                                                    const __grid_constant__ FeedFrameSet dst, int N, int C,
                                                     float unbiased) {
+    const FeedFramePtrs& d = dst.f[blockIdx.y];
+    src += (long long)blockIdx.y * N;
     const long long CN = (long long)C * N;
     for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < CN || t < N;
          t += (long long)gridDim.x * blockDim.x) {
@@ -42,25 +51,29 @@ __global__ void __launch_bounds__(256) k_feed_nodes(const fslic_cluster* __restr
             o.is_active = 0;
             o.is_updatable = 0;
             o.num_members = (uint32_t)feed_x86_trunc_i32((double)s.num_members);
-            dst.clusters[t] = o;
+            d.clusters[t] = o;
         }
         if (t < CN) {
-            dst.unary[t] = unbiased;
-            dst.q0[t] = 0.0f;
-            dst.q1[t] = 0.0f;
+            d.unary[t] = unbiased;
+            d.q0[t] = 0.0f;
+            d.q1[t] = 0.0f;
         }
     }
 }
 
-// counts[K] / neighbors[K][12] of the batch graph -> the frame's CSR: offsets = exclusive scan of the counts, the
-// neighbours row by row in list order (what set_connectivity makes of a NodeConnectivity).  One CTA of
-// FEED_CSR_THREADS; thread t owns the contiguous rows [t * per, (t + 1) * per).
+// counts[K] / neighbors[K][12] of graph blockIdx.y of the batch -> frame blockIdx.y's CSR: offsets = exclusive scan of
+// the counts, the neighbours row by row in list order (what set_connectivity makes of a NodeConnectivity).  One CTA of
+// FEED_CSR_THREADS per frame; thread t owns the contiguous rows [t * per, (t + 1) * per).
 #define FEED_CSR_THREADS 1024
 __global__ void __launch_bounds__(FEED_CSR_THREADS) k_feed_csr(const int32_t* __restrict__ counts,
                                                                const uint32_t* __restrict__ neighbors, int K,
-                                                               int32_t* __restrict__ offsets, int32_t* __restrict__ nbr) {
+                                                               const __grid_constant__ FeedFrameSet dst) {
     typedef cub::BlockScan<int, FEED_CSR_THREADS> Scan;
     __shared__ typename Scan::TempStorage scan_tmp;
+    counts += (long long)blockIdx.y * K;
+    neighbors += (long long)blockIdx.y * K * CONN_MAX;
+    int32_t* __restrict__ offsets = dst.f[blockIdx.y].offsets;
+    int32_t* __restrict__ nbr = dst.f[blockIdx.y].nbr;
     const int per = (K + FEED_CSR_THREADS - 1) / FEED_CSR_THREADS;
     const int r0 = min(K, (int)threadIdx.x * per), r1 = min(K, r0 + per);
     int own = 0;
@@ -76,8 +89,12 @@ __global__ void __launch_bounds__(FEED_CSR_THREADS) k_feed_csr(const int32_t* __
     }
 }
 
-// set_proba: unary = -logf(p), glibc's logf and x86's sign flip
-__global__ void __launch_bounds__(256) k_feed_proba(const float* __restrict__ p, float* __restrict__ unary, long long n) {
+// set_proba of frame blockIdx.y from p[blockIdx.y] (n = C * N values each): unary = -logf(p), glibc's logf and x86's
+// sign flip.  Only the unary pointers of the set are used.
+__global__ void __launch_bounds__(256) k_feed_proba(const float* __restrict__ p, const __grid_constant__ CrfFrameQSet set,
+                                                    long long n) {
+    float* __restrict__ unary = set.f[blockIdx.y].unary;
+    p += (long long)blockIdx.y * n;
     for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (long long)gridDim.x * blockDim.x)
         unary[k] = glogf::neg_logf(p[k]);
 }

@@ -370,6 +370,33 @@ int fslic_b200_crfdev_set_proba(fslic_crf* crf, int time, const float* d_proba, 
 int fslic_b200_crfdev_set_mask(fslic_crf* crf, int time, const int32_t* d_classes, float confidence, void* stream);
 int fslic_b200_crfdev_get_inferred(fslic_crf* crf, int time, float* d_out, void* stream);
 
+/* ---- Groups: the CRFs of many video streams driven together.  crfs[0 .. n) are n distinct CRFs on one device with
+ * the same num_classes C and num_nodes N; each keeps its own frames, params and time chain, and every result equals
+ * what the member's own calls give, bit for bit.  The members of one call share each launch (up to 64 per launch set;
+ * larger groups take several on the same stream).  Every call checks all its arguments before it enqueues anything
+ * (a NULL or repeated member, mismatched device, C or N: FSLIC_EINVAL; for inference and the newest-frame calls, a
+ * member without frames: FSLIC_ENOFRAME), so a refused call changes no member.  Each call adopts `stream` for every
+ * member like fslic_b200_crf_inference, waiting once for each different stream they were on.  Afterwards every member
+ * is in the state its own calls would have left it in, and its own entry points carry on from there.  d_* buffers are
+ * device memory on the members' device; [n][C][N] buffers are float and hold member k's values at k. */
+/* max_iter Jacobi steps of every member: 1 + 2 max_iter launches per 64 members, no host wait.  No-op for max_iter 0. */
+int fslic_b200_crfgroup_inference(fslic_crf* const* crfs, int n, unsigned long long max_iter, void* stream);
+/* Frame k, built from d_labels[k] and d_clusters[k] as fslic_b200_crfdev_push_label_frames builds it, is appended to
+ * crfs[k]; one adjacency-graph pass over the n maps.  d_scratch as fslic_b200_crfdev_push_scratch_bytes(K, n) says.
+ * times_out [n] (host, may be NULL) receives the new times.  One host wait, for the members' frame-table uploads. */
+int fslic_b200_crfdev_group_push_label_frames(fslic_crf* const* crfs, int n, int H, int W, int K,
+                                              const uint16_t* d_labels, const fslic_cluster* d_clusters,
+                                              void* d_scratch, size_t scratch_bytes, void* stream, int* times_out);
+/* set_proba (-logf(p)) of the newest frame of each member from d_proba [n][C][N] */
+int fslic_b200_crfdev_group_set_proba(fslic_crf* const* crfs, int n, const float* d_proba, void* stream);
+/* reset_inferred (q = expf(-unary)) of the newest frame of each member */
+int fslic_b200_crfdev_group_reset_inferred(fslic_crf* const* crfs, int n, void* stream);
+/* q of the newest frame of each member into d_out [n][C][N] */
+int fslic_b200_crfdev_group_get_inferred(fslic_crf* const* crfs, int n, float* d_out, void* stream);
+/* pop_frame of every member: times_out[k] (host, may be NULL) = the popped time, -1 for a member without frames.  One
+ * host wait per stream the members are on. */
+int fslic_b200_crfgroup_pop_frame(fslic_crf* const* crfs, int n, int* times_out);
+
 /* glibc's logf as the device feed evaluates it (fast_slic_b200/csrc/glibc_logf.cuh), like the expf pair above. */
 int fslic_b200_debug_logf_host(uint32_t first, long long n, float* h_out);
 int fslic_b200_debug_logf_device(int device, uint32_t first, long long n, float* d_out, void* stream);
