@@ -37,6 +37,8 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_debug_logf_host", "fslic_b200_debug_logf_device",
     "fslic_b200_crfgroup_inference", "fslic_b200_crfdev_group_push_label_frames", "fslic_b200_crfdev_group_set_proba",
     "fslic_b200_crfdev_group_reset_inferred", "fslic_b200_crfdev_group_get_inferred", "fslic_b200_crfgroup_pop_frame",
+    "fslic_b200_pool_batch_scratch_bytes", "fslic_b200_pool_batch", "fslic_b200_pool_unpool_batch",
+    "fslic_b200_pool_paint_argmax_batch",
 )
 
 STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity", "iterate")
@@ -115,6 +117,11 @@ def lib():
     L.fslic_b200_get_connectivity_batch.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, C.c_size_t, vp]
     L.fslic_b200_get_mask_density_batch.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
     L.fslic_b200_cluster_density_to_mask_batch.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp]
+    L.fslic_b200_pool_batch_scratch_bytes.argtypes = [i32, i32, i32, i32]
+    L.fslic_b200_pool_batch_scratch_bytes.restype = C.c_size_t
+    L.fslic_b200_pool_batch.argtypes = [i32, i32, i32, i32, i32, i32, vp, vp, i32, vp, vp, vp, C.c_size_t, vp]
+    L.fslic_b200_pool_unpool_batch.argtypes = [i32, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp]
+    L.fslic_b200_pool_paint_argmax_batch.argtypes = [i32, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp]
     L.fslic_b200_assign_kernel_time.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]
     L.fslic_b200_debug_cca_counters.argtypes = [vp, C.POINTER(C.c_int32), i32]
     L.fslic_b200_debug_select_profile.argtypes = [vp, C.POINTER(C.c_longlong), i32]

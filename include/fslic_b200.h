@@ -219,6 +219,27 @@ int fslic_b200_get_mask_density_batch(int device, int batch, int H, int W, int K
 int fslic_b200_cluster_density_to_mask_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels,
                                              const uint8_t* d_densities, uint8_t* d_result, void* stream);
 
+/* Superpixel pooling (pool.cuh; no counterpart in the reference) over `batch` label maps d_labels u16[B,H,W]: a label
+ * outside [0, K) belongs to no superpixel; 1 <= K <= 65534, C >= 1.  Asynchronous on `stream`, never synchronise, no
+ * float atomics: each image's result depends only on its own labels and features (DESIGN.md section 4.12 gives the
+ * summation order).  batch, H or W == 0 does nothing.
+ * Scratch bytes fslic_b200_pool_batch takes for one call: 16 per pixel, 8 per superpixel and the radix sort's temporary
+ * storage; 256 for no pixel; (size_t)-1 for a bad K or when batch * H * W > 2^31 - 1 or batch > 65536 (split the batch). */
+size_t fslic_b200_pool_batch_scratch_bytes(int batch, int H, int W, int K);
+/* d_features f32[B,C,H,W] -> d_out f32[B,C,K]: the sum over each superpixel's pixels, or with `mean` != 0 the sum divided
+ * by the pixel count (0 for an empty superpixel); d_counts int32[B,K]: the pixel counts of the label map. */
+int fslic_b200_pool_batch(int device, int batch, int H, int W, int C, int K, const uint16_t* d_labels,
+                          const float* d_features, int mean, float* d_out, int32_t* d_counts, void* d_scratch,
+                          size_t scratch_bytes, void* stream);
+/* d_values f32[B,C,K] -> d_out f32[B,C,H,W]: each pixel's superpixel value, divided by (float)d_divisor[b,label] when
+ * d_divisor (int32[B,K]) is not NULL; 0 where the label is outside [0, K). */
+int fslic_b200_pool_unpool_batch(int device, int batch, int H, int W, int C, int K, const uint16_t* d_labels,
+                                 const float* d_values, const int32_t* d_divisor, float* d_out, void* stream);
+/* d_q f32[B,C,K] -> d_out int16[B,H,W]: the first index of the maximum of q over C at each pixel's superpixel (a NaN
+ * counts as the maximum), -1 where the label is outside [0, K); C <= 32767.  d_node_class: int32[B,K] scratch. */
+int fslic_b200_pool_paint_argmax_batch(int device, int batch, int H, int W, int C, int K, const uint16_t* d_labels,
+                                       const float* d_q, int32_t* d_node_class, int16_t* d_out, void* stream);
+
 /* Stage probes for the parity tests (the reference's protected quad_image / assignment,
  * context.h:48-50): copies of the last iterate()'s Lab quad image [B,H,W,4] u8 and pre-CCA
  * labels [B,H,W] u16 into caller device buffers (either may be NULL). */
