@@ -33,5 +33,15 @@ __device__ __forceinline__ uint32_t ld_nc_u32(const uint32_t* p) {
     return v;
 }
 
+// Slot hash of a label-pair key (a << 16 | b) in the open-addressing pair tables (graph.cuh, rag.cuh)
+__device__ __forceinline__ uint32_t conn_hash(uint32_t key) {
+    key ^= key >> 15;
+    key *= 0x2c1b3c6du;
+    key ^= key >> 12;
+    key *= 0x297a2d39u;
+    key ^= key >> 15;
+    return key;
+}
+
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }

@@ -28,15 +28,6 @@
 //                     of distinct adjacent pairs) one thread replays the reference's loop itself over all pixels --
 //                     slow, exact, never needed for superpixel maps -- chosen on the device from the image's flag.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t conn_hash(uint32_t key) {
-    key ^= key >> 15;
-    key *= 0x2c1b3c6du;
-    key ^= key >> 12;
-    key *= 0x297a2d39u;
-    key ^= key >> 15;
-    return key;
-}
-
 __global__ void __launch_bounds__(256) k_connb_init(uint32_t* __restrict__ tkey, unsigned long long* __restrict__ tord,
                                                      long nslots, int tshift, int obits, int batch, int* __restrict__ overflow) {
     const unsigned long long omax = (1ull << obits) - 1ull;

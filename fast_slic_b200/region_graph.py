@@ -1,0 +1,146 @@
+"""Region adjacency graphs of superpixel label maps on the GPU (csrc/rag.cuh): for a batch of the int16 label maps
+iterate_batch returns, every pair of superpixels that touch, weighted by the length of their shared boundary, in the
+CSR / COO layout graph libraries take.  With pooling.pool it gives a superpixel GNN its node features and its graph::
+
+    x = pool(features, labels, K)                        # [B,C,K] node features
+    g = region_adjacency(labels, K)                      # the B*K nodes' graph, one block per image
+    A = torch.sparse_csr_tensor(g.indptr, g.edge_index[1], g.boundary.float(), (B * K, B * K))
+
+No counterpart in the reference: its get_connectivity keeps at most 12 neighbours per superpixel, in scan order, and
+is kept for parity with it.  DESIGN.md section 4.13 describes the kernels.
+"""
+import collections
+import operator
+
+import torch
+
+from . import _lib
+from .pooling import _check_K, _tensor  # the K range of pooling.MAX_K
+
+# Device memory the pair tables of one count launch take at most (8 bytes per slot, a power of two >= max(4096, 32 K)
+# slots per image): a batch that needs more runs in chunks of images, with identical results.
+RAG_SCRATCH_CAP = 1 << 30
+# Larger images could have a boundary count above int32
+MAX_PIXELS = 1 << 29
+_INT_MAX = 2 ** 31 - 1
+_NO_SIZE = 2 ** 64 - 1
+
+RegionGraph = collections.namedtuple("RegionGraph", ["indptr", "edge_index", "boundary"])
+
+
+def rag_chunk(B, H, W, K, connectivity):
+    """Images per count launch: as many as fit RAG_SCRATCH_CAP, at least one."""
+    f = _lib.lib().fslic_b200_rag_batch_scratch_bytes
+    one = int(f(1, H, W, K, connectivity, 0))
+    if one == _NO_SIZE:
+        raise ValueError("an image of %dx%d pixels is too large for a region adjacency graph" % (H, W))
+    c = max(1, min(B, RAG_SCRATCH_CAP // max(1, one)))
+    while c > 1:
+        nbytes = int(f(c, H, W, K, connectivity, 0))
+        if nbytes <= RAG_SCRATCH_CAP:
+            break
+        c = max(1, min(c - 1, c * RAG_SCRATCH_CAP // nbytes))
+    return c
+
+
+def _split(b0, flags):
+    """The images of a count whose tables overflowed, each on its own with an exact table, and the runs between them
+    with the usual one: (first image, images, exact) in batch order."""
+    runs, start = [], 0
+    for i, flag in enumerate(flags + [1]):
+        if flag:
+            if i > start:
+                runs.append((b0 + start, i - start, 0))
+            if i < len(flags):
+                runs.append((b0 + i, 1, 1))
+            start = i + 1
+    return runs
+
+
+def region_adjacency(labels, K, connectivity=4):
+    """Region adjacency graph of int16 labels [B,H,W] (read as uint16) -> RegionGraph(indptr, edge_index, boundary).
+
+    Node n = b*K + k is label k of image b; no edge joins two images (the block-diagonal batch graph of PyG's Batch).
+    - indptr     int64 [B*K + 1]: CSR row offsets; node n's edges are indptr[n]:indptr[n+1].
+    - edge_index int64 [2, E]: (source, target) of both directions of every edge, sorted by source then target, so
+      edge_index[1] is the CSR column array.
+    - boundary   int32 [E]: the number of adjacent pixel pairs whose labels are the edge's two nodes.
+    Pixel pairs are the horizontally and vertically adjacent pixels (connectivity=4), plus both diagonals
+    (connectivity=8), each unordered pair once, the last row and column included.  A label outside [0, K) (-1 included)
+    belongs to no node and its pairs are ignored; a pair with equal labels is no edge.  1 <= K <= 65534 and
+    H * W <= 2^29; anything else, a tensor that is not a cuda int16 [B,H,W] tensor, or a connectivity other than 4 or 8
+    raises ValueError before any device work.  B, H or W = 0 gives zero rows and no edges.
+
+    Work runs on the labels' device, on its current stream.  The edge count is data-dependent, so, like torch.unique,
+    this call waits for the device: it reads (images + 1) int64 words back once per chunk of images (the edge total
+    and which images' pair tables overflowed; such images are counted again with an exact table, one read more per
+    run of images recounted -- only label maps that are not superpixel maps, such as noise, need that).  It cannot be
+    captured in a CUDA graph and raises RuntimeError under capture, before any device work.  All arithmetic is
+    integer: the result is exact and the same across runs, batch order, chunking and streams."""
+    _tensor("labels", labels, torch.int16, 3)
+    try:
+        connectivity = operator.index(connectivity)
+    except TypeError:
+        raise ValueError("connectivity must be 4 or 8, got %r" % (connectivity,)) from None
+    if connectivity not in (4, 8):
+        raise ValueError("connectivity must be 4 or 8, got %r" % (connectivity,))
+    K = _check_K(K)
+    B, H, W = (int(v) for v in labels.shape)
+    if H * W > MAX_PIXELS:
+        raise ValueError("images of %dx%d pixels exceed %d pixels: a boundary count could overflow int32"
+                         % (H, W, MAX_PIXELS))
+    if labels.device.type != "cuda":
+        raise ValueError("labels is a %s tensor: pass cuda tensors (torch.from_numpy(...).cuda())" % labels.device.type)
+    dev = labels.device
+    with torch.cuda.device(dev):
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("region_adjacency reads its edge count back to the host and cannot be captured in a "
+                               "CUDA graph")
+        if B == 0 or H == 0 or W == 0:
+            return RegionGraph(torch.zeros(B * K + 1, dtype=torch.int64, device=dev),
+                               torch.empty((2, 0), dtype=torch.int64, device=dev),
+                               torch.empty(0, dtype=torch.int32, device=dev))
+        lab = labels.contiguous()
+        L = _lib.lib()
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        indptr = torch.empty(B * K + 1, dtype=torch.int64, device=dev)
+        chunk = rag_chunk(B, H, W, K, connectivity)
+        work = [(b0, min(chunk, B - b0), 0) for b0 in range(0, B, chunk)][::-1]
+        pieces, edges = [], 0
+        while work:
+            b0, c, exact = work.pop()
+            nbytes = int(L.fslic_b200_rag_batch_scratch_bytes(c, H, W, K, connectivity, exact))
+            if nbytes == _NO_SIZE:
+                raise MemoryError("image %d has too many distinct adjacent label pairs for an exact pair table" % b0)
+            scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            info = torch.empty(c + 1, dtype=torch.int64, device=dev)
+            _lib.check(L.fslic_b200_rag_batch_count(dev.index, c, H, W, K, connectivity, exact, lab[b0].data_ptr(), edges,
+                                                    indptr[b0 * K:].data_ptr(), info.data_ptr(), scratch.data_ptr(),
+                                                    nbytes, stream))
+            info = info.tolist()  # the host wait: overflow flags and the edge total
+            flags, total = info[:c], info[c]
+            if any(flags):
+                work.extend(_split(b0, flags)[::-1])
+                continue
+            if total > _INT_MAX:  # one segmented sort per fill
+                if c == 1:
+                    raise MemoryError("image %d has %d directed edges, more than one fill takes" % (b0, total))
+                work.extend([(b0 + c // 2, c - c // 2, exact), (b0, c // 2, exact)])
+                continue
+            edge_index = torch.empty((2, total), dtype=torch.int64, device=dev)
+            boundary = torch.empty(total, dtype=torch.int32, device=dev)
+            if total:
+                fbytes = int(L.fslic_b200_rag_fill_scratch_bytes(c, K, total))
+                fill = torch.empty(fbytes, dtype=torch.uint8, device=dev)
+                _lib.check(L.fslic_b200_rag_batch_fill(dev.index, c, H, W, K, connectivity, exact, b0 * K, total,
+                                                       scratch.data_ptr(), nbytes, fill.data_ptr(), fbytes,
+                                                       edge_index[0].data_ptr(), edge_index[1].data_ptr(),
+                                                       boundary.data_ptr(), stream))
+            pieces.append((edge_index, boundary))
+            edges += total
+        if len(pieces) == 1:
+            edge_index, boundary = pieces[0]
+        else:
+            edge_index = torch.cat([p[0] for p in pieces], dim=1)
+            boundary = torch.cat([p[1] for p in pieces])
+    return RegionGraph(indptr, edge_index, boundary)

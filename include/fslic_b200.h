@@ -240,6 +240,34 @@ int fslic_b200_pool_unpool_batch(int device, int batch, int H, int W, int C, int
 int fslic_b200_pool_paint_argmax_batch(int device, int batch, int H, int W, int C, int K, const uint16_t* d_labels,
                                        const float* d_q, int32_t* d_node_class, int16_t* d_out, void* stream);
 
+/* Region adjacency graphs (rag.cuh; no counterpart in the reference) of `batch` label maps d_labels u16[B,H,W]: node
+ * b*K + k is label k of image b; an edge joins two labels of one image for every unordered pair of adjacent pixels
+ * (connectivity 4: horizontal and vertical neighbours; 8: also both diagonals) that carry them, and its weight is the
+ * number of such pixel pairs.  A label outside [0, K) belongs to no node.  1 <= K <= 65534, H * W <= 2^29.  Two calls
+ * per batch, asynchronous on `stream`, never synchronise: the count writes the CSR row offsets and the edge total, the
+ * caller reads the total back and allocates the edges, the fill writes them (DESIGN.md section 4.13).
+ * Scratch bytes of the count (the fill reads it too): 8 per pair-table slot, 16 per node and the scan's temporary
+ * storage.  Each image's table has T slots, a power of two: with `exact`, T >= 2 * min(K (K - 1) / 2, pixel pairs of
+ * the image), which cannot overflow; else the smaller of that and max(4096, 32 K), which can.  256 for no pixel;
+ * (size_t)-1 for bad arguments, H * W > 2^29, B * K >= 2^31 - 1 or an exact table over 2^31 slots. */
+size_t fslic_b200_rag_batch_scratch_bytes(int batch, int H, int W, int K, int connectivity, int exact);
+/* d_indptr int64[B*K + 1]: edge_base + the exclusive sum of the node degrees; d_info int64[B + 1]: d_info[b] = 1 where
+ * image b's table overflowed (its edges are incomplete: count it again with `exact`), d_info[B] = the directed edge
+ * total E of the call. */
+int fslic_b200_rag_batch_count(int device, int batch, int H, int W, int K, int connectivity, int exact,
+                               const uint16_t* d_labels, long long edge_base, long long* d_indptr, long long* d_info,
+                               void* d_scratch, size_t scratch_bytes, void* stream);
+/* Scratch bytes of the fill for E edges: 20 per edge and the radix sort's temporary storage; 256 for E = 0;
+ * (size_t)-1 for E > 2^31 - 1 (split the batch). */
+size_t fslic_b200_rag_fill_scratch_bytes(int batch, int K, long long edges);
+/* After a count with the same batch, H, W, K, connectivity, exact and d_scratch, and `edges` = its d_info[B]:
+ * d_src / d_dst int64[E] (node ids + node_base) and d_boundary int32[E], both directions of every edge, rows in
+ * source order, each row sorted by target. */
+int fslic_b200_rag_batch_fill(int device, int batch, int H, int W, int K, int connectivity, int exact,
+                              long long node_base, long long edges, const void* d_scratch, size_t scratch_bytes,
+                              void* d_fill_scratch, size_t fill_bytes, long long* d_src, long long* d_dst,
+                              int32_t* d_boundary, void* stream);
+
 /* Stage probes for the parity tests (the reference's protected quad_image / assignment,
  * context.h:48-50): copies of the last iterate()'s Lab quad image [B,H,W,4] u8 and pre-CCA
  * labels [B,H,W] u16 into caller device buffers (either may be NULL). */
