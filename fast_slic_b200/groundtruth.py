@@ -1,0 +1,179 @@
+"""Superpixels against ground truth on the GPU (csrc/groundtruth.cuh), for whole batches of the int16 label maps
+iterate_batch returns: per-superpixel class histograms (the node targets of a superpixel classifier or GNN), the
+standard superpixel quality scores (achievable segmentation accuracy, undersegmentation error, boundary recall and
+precision within a pixel tolerance) and the boundary map of a label map.  With pooling.pool and
+region_graph.region_adjacency it gives a superpixel GNN its targets::
+
+    x = pool(features, labels, K)                                           # [B,C,K] node features
+    g = region_adjacency(labels, K)                                         # their graph
+    h = class_histogram(seg, labels, K, num_classes)                        # seg: [B,H,W] class map -> int32 [B,K,C]
+    y = torch.where(h.sum(-1) > 0, h.argmax(-1), -100).reshape(-1)          # [B*K] targets; -100: CrossEntropyLoss's
+                                                                            # ignore_index for empty superpixels
+
+(argmax picks the lowest class on ties.)  No counterpart in the reference.  Cuda tensors only: labels int16 [B,H,W],
+read as uint16, and a class / gt map of the same shape, uint8, int16, int32 or int64.  Every argument is checked
+(ValueError) before any device work.  Work runs on the labels' device, on its current stream, and nothing is read back
+to the host, so a CUDA graph can capture every call.  All arithmetic is integer: image b's result depends only on
+labels[b] and gt[b] -- not on the batch, its place in it, the chunking, the stream or the run.  DESIGN.md section 4.14
+describes the kernels.
+"""
+import collections
+import operator
+
+import torch
+
+from . import _lib
+from .pooling import _check_K, _devices, _tensor
+from .region_graph import MAX_PIXELS
+
+# Device memory one scores launch takes at most (about 20.4 bytes per pixel and 16 per superpixel, plus the sort's
+# storage): a batch that needs more runs in chunks of images, with identical results.
+GT_SCRATCH_CAP = 1 << 30
+MAX_CLASSES = 65536
+MAX_TOLERANCE = 32
+_MAX_CHUNK = 1 << 17  # the image bits of an overlap key
+_INT64 = (-2 ** 63, 2 ** 63 - 1)
+# the FSLIC_GT_* codes of include/fslic_b200.h: the element size
+_DTYPES = {torch.uint8: 1, torch.int16: 2, torch.int32: 4, torch.int64: 8}
+
+SegmentationScores = collections.namedtuple("SegmentationScores", [
+    "pixels", "asa_pixels", "ue_pixels", "gt_boundary", "gt_boundary_hits", "sp_boundary", "sp_boundary_hits",
+    "asa", "undersegmentation", "boundary_recall", "boundary_precision"])
+
+
+def _int(name, v, lo, hi):
+    try:
+        v = operator.index(v)
+    except TypeError:
+        raise ValueError("%s must be an int, got %r" % (name, v)) from None
+    if not lo <= v <= hi:
+        raise ValueError("%s must be in [%d, %d], got %d" % (name, lo, hi, v))
+    return v
+
+
+def _check(name, gt, labels):
+    """labels: int16 [B,H,W]; gt: a [B,H,W] map of a _DTYPES dtype; images of at most MAX_PIXELS pixels.  Returns
+    (B, H, W)."""
+    _tensor("labels", labels, torch.int16, 3)
+    if not isinstance(gt, torch.Tensor):
+        raise ValueError("%s must be a cuda tensor (got %s): use torch.from_numpy(...).cuda()" % (name, type(gt).__name__))
+    if gt.dtype not in _DTYPES:
+        raise ValueError("%s must be a uint8, int16, int32 or int64 tensor, got %s" % (name, gt.dtype))
+    if tuple(gt.shape) != tuple(labels.shape):
+        raise ValueError("%s %s does not match labels %s" % (name, tuple(gt.shape), tuple(labels.shape)))
+    B, H, W = (int(v) for v in labels.shape)
+    if H * W > MAX_PIXELS:
+        raise ValueError("images of %dx%d pixels exceed %d pixels: a count could overflow int32" % (H, W, MAX_PIXELS))
+    return B, H, W
+
+
+def class_histogram(classes, labels, K, num_classes):
+    """Class map classes [B,H,W] (uint8, int16, int32 or int64), int16 labels [B,H,W] (read as uint16) -> int32
+    [B, K, num_classes]: out[b, k, c] is the number of pixels of image b with label k and class c.  A pixel whose label
+    is outside [0, K) (-1 included) or whose class is outside [0, num_classes) (such as the ignore values 255 or -1) is
+    not counted.  1 <= K <= 65534, 1 <= num_classes <= 65536.
+
+    The majority class of each superpixel, as node targets (argmax picks the lowest class on ties; -100 is
+    CrossEntropyLoss's ignore_index, for superpixels with no counted pixel)::
+
+        h = class_histogram(seg, labels, K, C)
+        y = torch.where(h.sum(-1) > 0, h.argmax(-1), -100).reshape(-1)     # [B*K]
+    """
+    B, H, W = _check("classes", classes, labels)
+    K = _check_K(K)
+    C = _int("num_classes", num_classes, 1, MAX_CLASSES)
+    dev = _devices(labels, "classes", classes)
+    with torch.cuda.device(dev):
+        out = torch.empty((B, K, C), dtype=torch.int32, device=dev)
+        if B == 0 or H == 0 or W == 0:
+            return out.zero_()
+        cls, lab = classes.contiguous(), labels.contiguous()
+        _lib.check(_lib.lib().fslic_b200_gt_histogram_batch(
+            dev.index, B, H, W, K, C, _DTYPES[cls.dtype], cls.data_ptr(), lab.data_ptr(), out.data_ptr(),
+            torch.cuda.current_stream(dev).cuda_stream))
+    return out
+
+
+def gt_chunk(B, H, W, K):
+    """Images per scores launch: as many as fit GT_SCRATCH_CAP, at least one."""
+    f = _lib.lib().fslic_b200_gt_scores_scratch_bytes
+    one = int(f(1, H, W, K))
+    if one == 2 ** 64 - 1:
+        raise ValueError("an image of %dx%d pixels is too large to score" % (H, W))
+    c = max(1, min(B, _MAX_CHUNK, GT_SCRATCH_CAP // max(1, one)))
+    while c > 1:
+        nbytes = int(f(c, H, W, K))
+        if nbytes <= GT_SCRATCH_CAP:
+            break
+        c = max(1, min(c - 1, c * GT_SCRATCH_CAP // nbytes))
+    return c
+
+
+def _ratio(num, den):
+    return torch.where(den > 0, num.double() / den.double(), torch.full_like(num, float("nan"), dtype=torch.float64))
+
+
+def segmentation_scores(labels, gt, K, tolerance=2, ignore_index=None):
+    """Scores of int16 superpixel labels [B,H,W] (read as uint16) against a ground-truth segmentation gt [B,H,W]
+    (uint8, int16, int32 or int64) -> SegmentationScores, every field a [B] tensor on the labels' device.
+
+    A gt pixel is valid when 0 <= gt <= 2^31 - 1 and gt != ignore_index; a pixel is counted when it is valid and its
+    label is in [0, K).  n_kg is the number of counted pixels of an image with label k and gt value g, n_k = sum_g n_kg.
+    Integer fields (int64), exact, so that dataset totals can be summed over images before dividing:
+    - pixels: the counted pixels N;
+    - asa_pixels: sum_k max_g n_kg;
+    - ue_pixels: the sum over the pairs with n_kg > 0 of min(n_kg, n_k - n_kg) (Neubert and Protzel's corrected
+      undersegmentation error);
+    - gt_boundary: the gt boundary pixels, valid pixels whose right or lower neighbour is valid and has another gt value;
+    - gt_boundary_hits: those with a superpixel boundary pixel (see boundaries) in their window;
+    - sp_boundary: the superpixel boundary pixels that are valid in gt;
+    - sp_boundary_hits: those with a gt boundary pixel in their window.
+    The window of a pixel is the square |di|, |dj| <= tolerance (an int in [0, 32]) clipped to the image.  This is the
+    common fast form of boundary recall, not the BSDS bipartite matching of boundary pixels.
+    Ratios (float64, NaN where the denominator is 0): asa = asa_pixels / pixels, undersegmentation = ue_pixels /
+    pixels, boundary_recall = gt_boundary_hits / gt_boundary, boundary_precision = sp_boundary_hits / sp_boundary.
+
+    For several annotations per image, as in BSDS, stack them along B and repeat the labels to match
+    (labels.repeat_interleave(A, 0) for A annotations per image)."""
+    B, H, W = _check("gt", gt, labels)
+    K = _check_K(K)
+    r = _int("tolerance", tolerance, 0, MAX_TOLERANCE)
+    ignore = None if ignore_index is None else _int("ignore_index", ignore_index, *_INT64)
+    dev = _devices(labels, "gt", gt)
+    with torch.cuda.device(dev):
+        out = torch.zeros((B, 7), dtype=torch.int64, device=dev)
+        if B and H and W:
+            g, lab = gt.contiguous(), labels.contiguous()
+            L = _lib.lib()
+            chunk = gt_chunk(B, H, W, K)
+            nbytes = int(L.fslic_b200_gt_scores_scratch_bytes(chunk, H, W, K))
+            scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            for b0 in range(0, B, chunk):
+                c = min(chunk, B - b0)
+                _lib.check(L.fslic_b200_gt_scores_batch(
+                    dev.index, c, H, W, K, r, _DTYPES[g.dtype], g[b0].data_ptr(), lab[b0].data_ptr(),
+                    int(ignore is not None), 0 if ignore is None else ignore, out[b0].data_ptr(), scratch.data_ptr(),
+                    nbytes, stream))
+        f = out.t().contiguous().unbind(0)
+        return SegmentationScores(*f, _ratio(f[1], f[0]), _ratio(f[2], f[0]), _ratio(f[4], f[3]), _ratio(f[6], f[5]))
+
+
+def boundaries(labels):
+    """int16 labels [B,H,W] -> bool [B,H,W]: True at superpixel boundary pixels, those whose right or lower neighbour
+    exists and carries another raw label -- a one-sided, 1-pixel-wide outline (what skimage's mark_boundaries draws),
+    the same predicate segmentation_scores uses."""
+    _tensor("labels", labels, torch.int16, 3)
+    B, H, W = (int(v) for v in labels.shape)
+    if H * W > MAX_PIXELS:
+        raise ValueError("images of %dx%d pixels exceed %d pixels" % (H, W, MAX_PIXELS))
+    if labels.device.type != "cuda":
+        raise ValueError("labels is a %s tensor: pass cuda tensors (torch.from_numpy(...).cuda())" % labels.device.type)
+    dev = labels.device
+    with torch.cuda.device(dev):
+        out = torch.empty((B, H, W), dtype=torch.bool, device=dev)
+        if B and H and W:
+            lab = labels.contiguous()
+            _lib.check(_lib.lib().fslic_b200_gt_boundaries_batch(dev.index, B, H, W, lab.data_ptr(), out.data_ptr(),
+                                                                 torch.cuda.current_stream(dev).cuda_stream))
+    return out

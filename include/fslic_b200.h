@@ -268,6 +268,35 @@ int fslic_b200_rag_batch_fill(int device, int batch, int H, int W, int K, int co
                               void* d_fill_scratch, size_t fill_bytes, long long* d_src, long long* d_dst,
                               int32_t* d_boundary, void* stream);
 
+/* Superpixels scored against ground truth (groundtruth.cuh; no counterpart in the reference) over `batch` label maps
+ * d_labels u16[B,H,W] and maps of the same shape whose element type is `dtype`, one of the FSLIC_GT_* codes (the element
+ * size in bytes).  A label outside [0, K) belongs to no superpixel; 1 <= K <= 65534, H * W <= 2^29.  Integer only,
+ * asynchronous on `stream`, never synchronise (a CUDA graph can capture them); batch, H or W == 0 launches nothing.
+ * DESIGN.md section 4.14 gives the definitions. */
+#define FSLIC_GT_UINT8 1
+#define FSLIC_GT_INT16 2
+#define FSLIC_GT_INT32 4
+#define FSLIC_GT_INT64 8
+/* d_out int32[B,K,C] (C = num_classes, 1..65536): the number of pixels of image b with label k and class c; pixels with
+ * a label outside [0, K) or a class outside [0, C) are not counted. */
+int fslic_b200_gt_histogram_batch(int device, int batch, int H, int W, int K, int num_classes, int dtype,
+                                  const void* d_classes, const uint16_t* d_labels, int32_t* d_out, void* stream);
+/* Scratch bytes of one fslic_b200_gt_scores_batch call: 20 per pixel for the overlap keys and runs, 3/8 per pixel for
+ * the boundary bitmaps, 16 per (image, label) and the larger temporary storage of the radix sort and the run-length
+ * encoding; 256 for no pixel; (size_t)-1 for bad arguments or when batch * H * W > 2^31 - 1 or batch > 2^17 (split the
+ * batch). */
+size_t fslic_b200_gt_scores_scratch_bytes(int batch, int H, int W, int K);
+/* d_out int64[B,7] per image: counted pixels, the ASA numerator sum_k max_g n_kg, the UE numerator
+ * sum_{k,g: n_kg > 0} min(n_kg, n_k - n_kg), gt boundary pixels, those with a superpixel boundary pixel within the
+ * Chebyshev `tolerance` (0..32), superpixel boundary pixels valid in gt, those with a gt boundary pixel within it.  A gt
+ * value is valid in [0, 2^31 - 1] and, with has_ignore, != ignore. */
+int fslic_b200_gt_scores_batch(int device, int batch, int H, int W, int K, int tolerance, int dtype, const void* d_gt,
+                               const uint16_t* d_labels, int has_ignore, long long ignore, long long* d_out,
+                               void* d_scratch, size_t scratch_bytes, void* stream);
+/* d_out u8[B,H,W]: 1 where the right or lower neighbour exists and carries another label, else 0. */
+int fslic_b200_gt_boundaries_batch(int device, int batch, int H, int W, const uint16_t* d_labels, uint8_t* d_out,
+                                   void* stream);
+
 /* Stage probes for the parity tests (the reference's protected quad_image / assignment,
  * context.h:48-50): copies of the last iterate()'s Lab quad image [B,H,W,4] u8 and pre-CCA
  * labels [B,H,W] u16 into caller device buffers (either may be NULL). */
