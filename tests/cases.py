@@ -236,6 +236,122 @@ def gpu_random_config_case(seed):
     return ("gpu_random%d" % seed, kind, H, W, K, dict(args, sigma=sigma)), 900 + seed
 
 
+# ---- seeded sweeps of the float-distance, preemptive, Euclidean and LSC contexts --------------------------------------
+# Wider than gpu_random_config_case: shapes from one row or column up to about 420 x 560 (widths that are and are not
+# multiples of 8), K from 1 up to one cluster per pixel, parameters at the ends of their ranges, flat images.  Every
+# sixth seed takes one regime of K: ordinary, dense (S = 1..3), S > 110, K > 4096, a one-row or one-column image.
+SWEEP_KINDS = ("syn", "noise", "blocks", "flat")
+SWEEP_COMPACTNESS = (0.01, 0.5, 3.0, 10.0, 40.0, 100.0)
+SWEEP_MSF = (0.0, 0.1, 0.25, 1.0, 3.0)
+SWEEP_STRIDES = (1, 2, 3, 5, 255)
+SWEEP_THRES = (0.01, 0.05, 0.2, 0.5, 1.0)
+K_MAX = 65533  # num_components < 65534 (cfast_slic.pyx:24-25)
+
+
+def sweep_S(H, W, K):
+    """The context's S (context.h:60: integer division first, then the square root, truncated)."""
+    return int(np.sqrt(float(H * W // K)))
+
+
+def sweep_turn(seed):
+    """What the image kind and the float-distance variant cycle with: the seed plus one per round of six regimes, so
+    that every regime meets every kind and variant (seed % 3 or seed % 4 alone would pair them with fixed regimes)."""
+    return seed + seed // 6
+
+
+def sweep_config(rng, seed):
+    """(kind, H, W, K, kwargs) of sweep seed `seed`, drawn from `rng`."""
+    regime = seed % 6
+
+    def width(lo, hi):
+        w = int(rng.randint(lo, hi + 1))
+        return max(8, w - w % 8) if rng.randint(2) else w
+
+    if regime == 1:    # dense: S = 1, 1, 2, 2 or 3
+        H, W = int(rng.randint(6, 121)), width(6, 160)
+        K = max(1, min(K_MAX, H * W // int(rng.choice([1, 2, 4, 6, 9]))))
+    elif regime == 2:  # S > 110: k_assign_real / k_assign_lsc windows wider than any tile kernel's
+        H, W = int(rng.randint(240, 421)), width(240, 560)
+        K = int(rng.randint(1, H * W // (111 * 111) + 1))
+    elif regime == 3:  # K > 4096: k_prepare instead of the in-tail prepare
+        H, W = int(rng.randint(100, 421)), width(100, 560)
+        K = int(rng.randint(4097, min(K_MAX, H * W // 2) + 1))
+    elif regime == 4:  # one row or one column
+        L = int(rng.randint(2, 561))
+        H, W = (1, L) if rng.randint(2) else (L, 1)
+        K = int(rng.randint(1, L // 2 + 1))
+    else:
+        H, W = int(rng.randint(1, 421)), width(1, 560)
+        K = int(rng.randint(1, max(2, H * W // 60)))
+    kind = SWEEP_KINDS[sweep_turn(seed) % 4]
+    args = dict(max_iter=0 if seed % 7 == 3 else int(rng.randint(1, 16)),
+                compactness=float(rng.choice(SWEEP_COMPACTNESS)), min_size_factor=float(rng.choice(SWEEP_MSF)),
+                subsample_stride=int(rng.choice(SWEEP_STRIDES)), convert_to_lab=bool(rng.randint(0, 2)),
+                sigma=float(rng.choice([5.0, 12.0, 30.0])))
+    return kind, H, W, K, args
+
+
+def real_sweep_case(seed, family=0):
+    """Float-distance sweep: ((kind, H, W, K, kwargs), variant).  family 0: the Manhattan sweep (variants 0, 1, 2 by
+    seed), 1: the Euclidean one (variants 0 and 2; "l2" ignores the flag)."""
+    rng = np.random.RandomState(11000 + 1000 * family + seed)
+    case = sweep_config(rng, seed)
+    return case, (sweep_turn(seed) % 3 if family == 0 else (0, 2)[sweep_turn(seed) % 2])
+
+
+def preempt_sweep_case(seed, family=0):
+    """preemptive=True sweep: (kind, H, W, K, thres, kwargs); family 0 Manhattan, 1 Euclidean."""
+    rng = np.random.RandomState(13008 + 1000 * family + seed)  # (a base at which both families reach every region)
+    kind, H, W, K, args = sweep_config(rng, seed)
+    return kind, H, W, K, float(rng.choice(SWEEP_THRES)), args
+
+
+def sweep_regions(case):
+    """The regions of the parameter space that the hand-picked case lists leave out and case (kind, H, W, K, [thres,]
+    kwargs) falls in."""
+    kind, H, W, K = case[:4]
+    S, a = sweep_S(H, W, K), split_kwargs(case[-1])[1]
+    long_run = a["subsample_stride"] == 1 or a["subsample_stride"] >= 5
+    return {name for name, hit in (
+        ("S <= 2", S <= 2), ("S > 110", S > 110), ("K > 4096", K > 4096), ("one row or column", H == 1 or W == 1),
+        ("W % 8 == 0", W % 8 == 0 and W > 1), ("W % 8 != 0", W % 8 != 0), ("stride 1", a["subsample_stride"] == 1),
+        ("stride >= 5", a["subsample_stride"] >= 5), ("max_iter 0", a["max_iter"] == 0),
+        ("max_iter >= 13", a["max_iter"] >= 13), ("stride 1 or >= 5 with max_iter 0 or >= 13",
+                                                 long_run and (a["max_iter"] == 0 or a["max_iter"] >= 13)),
+        ("Lab off", not a["convert_to_lab"]), ("Lab on", a["convert_to_lab"]), ("msf >= 1", a["min_size_factor"] >= 1),
+        ("compactness 0.01", a["compactness"] == 0.01), ("compactness 100", a["compactness"] == 100.0),
+        ("flat image", kind == "flat")) if hit}
+
+
+SWEEP_REGIONS = ("S <= 2", "S > 110", "K > 4096", "one row or column", "W % 8 == 0", "W % 8 != 0", "stride 1",
+                 "stride >= 5", "max_iter 0", "max_iter >= 13", "stride 1 or >= 5 with max_iter 0 or >= 13", "Lab off",
+                 "Lab on", "msf >= 1", "compactness 0.01", "compactness 100", "flat image")
+
+REAL_SWEEP_SEEDS = range(24)
+PREEMPT_SWEEP_SEEDS = range(16)
+
+
+def sweep_case_id(case):
+    """kind_HxW_K<K> plus the parameters that differ between seeds, for test ids."""
+    kind, H, W, K = case[:4]
+    a = split_kwargs(case[-1])[1]
+    return "%s_%dx%d_K%d_it%d_c%g_m%g_s%d%s" % (kind, H, W, K, a["max_iter"], a["compactness"], a["min_size_factor"],
+                                                 a["subsample_stride"], "" if a["convert_to_lab"] else "_rgb")
+
+
+def real_dist_sweep_outputs(impl, variant, case):
+    """real_dist_warm_outputs with the pre-CCA labels of both calls."""
+    kind, H, W, K, ckw = case
+    sigma, a = split_kwargs(ckw)
+    img = make_image(kind, H, W, seed=41, sigma=sigma)
+    cl = impl.initialize(img, K)
+    out = {}
+    for round_ in range(2):
+        lab, pre = impl.iterate_real(variant, img, cl, *_args(a), stages=True)
+        out.update({"pre%d" % round_: pre, "labels%d" % round_: lab, "clusters%d" % round_: cl.copy()})
+    return out
+
+
 def real_dist_warm_outputs(impl, variant, case):
     """A float-distance class called twice on one image (test_real_dist_variants): labels and clusters per call."""
     kind, H, W, K, ckw = case
@@ -302,6 +418,12 @@ def gpu_suite_cases():
     for case in GPU_PREEMPT_CASES:
         cases.append(("gpu_preempt/%s_%dx%d_K%d_t%g" % case[:5], lambda impl, c=case, **kw: preemptive_outputs(impl, c, **kw)))
     cases.append(("cca/gpu_suite", lambda impl, **kw: cca_outputs(impl, **kw)))
+    for seed in REAL_SWEEP_SEEDS:
+        case, variant = real_sweep_case(seed)
+        cases.append(("gpu_real_sweep/%d" % seed, lambda impl, v=variant, c=case, **kw: real_dist_sweep_outputs(impl, v, c)))
+    for seed in PREEMPT_SWEEP_SEEDS:
+        cases.append(("gpu_preempt_sweep/%d" % seed,
+                      lambda impl, c=preempt_sweep_case(seed), **kw: preemptive_outputs(impl, c, **kw)))
     return cases
 
 

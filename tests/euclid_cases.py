@@ -4,7 +4,8 @@ each one exercises the option (tests/test_euclidean_cpu.py checks that).
 
 The *_outputs functions run one case on `impl`: a checker of oracle_euclid.euclid (Euclidean) or of oracle.oracle (the
 same case with the Manhattan term, for comparison); `kw` are extra keyword arguments of its iterate call."""
-from cases import EDGE_CASES, PIPELINE_CASES, TMA_CASES, make_image, pipeline_outputs, split_kwargs
+from cases import (EDGE_CASES, PIPELINE_CASES, TMA_CASES, make_image, pipeline_outputs, preempt_sweep_case,
+                   real_sweep_case, split_kwargs)
 
 _BY_NAME = {c[0]: c for c in PIPELINE_CASES + EDGE_CASES + TMA_CASES}
 
@@ -38,6 +39,19 @@ EUCLID_PREEMPT_CASES = [("syn", 120, 160, 48, 0.05, {}), ("syn", 240, 320, 200, 
                         ("syn", 181, 257, 90, 0.1, dict(subsample_stride=1, max_iter=6)),
                         ("blocks", 240, 320, 64, 0.5, dict(subsample_stride=2))]
 EUCLID_ARCHS = ("x64/avx2", "standard")
+
+# seeded sweeps (tests/cases.py::sweep_config): float-distance variants 0 and 2, and preemptive.  Unlike the lists above
+# a sweep case need not change with the flag (flat images, max_iter 0, ...): it is a parity case only.
+EUCLID_REAL_SWEEP = [real_sweep_case(seed, family=1) for seed in range(12)]   # ((kind, H, W, K, kw), variant)
+EUCLID_PREEMPT_SWEEP = [preempt_sweep_case(seed, family=1) for seed in range(8)]
+
+
+def real_sweep_id(seed):
+    return "real_sweep/%d" % seed
+
+
+def preempt_sweep_id(seed):
+    return "preempt_sweep/%d" % seed
 
 
 def case_id(group, case):
@@ -98,8 +112,12 @@ def euclid_reference_outputs(impl, threads=2):
             euclid_pipeline_outputs(impl, "warm", EUCLID_WARM_CASE, 3, **kw)
         for case in EUCLID_PREEMPT_CASES:
             yield "%s/%s" % (top, preempt_case_id(case)), euclid_preempt_outputs(impl, case, **kw)
+        for seed, case in enumerate(EUCLID_PREEMPT_SWEEP):
+            yield "%s/%s" % (top, preempt_sweep_id(seed)), euclid_preempt_outputs(impl, case, **kw)
     for variant in (0, 2):
         for case in EUCLID_REAL_CASES:
             yield "euclid/" + real_case_id(variant, case), euclid_real_outputs(impl, variant, case, num_threads=threads)
     for case in EUCLID_L2_CASES:  # the "l2" context ignores the flag: these must equal its Manhattan outputs
         yield "euclid/" + real_case_id(1, case), euclid_real_outputs(impl, 1, case, num_threads=threads)
+    for seed, (case, variant) in enumerate(EUCLID_REAL_SWEEP):
+        yield "euclid/" + real_sweep_id(seed), euclid_real_outputs(impl, variant, case, num_threads=threads)

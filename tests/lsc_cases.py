@@ -3,7 +3,9 @@ tests/golden/make_lsc_golden.py.
 
 Each case runs one LSC context twice on one image: cold start from initialize_clusters, then warm start on the records
 the first call left ("...0" / "...1" outputs)."""
-from cases import make_image, split_kwargs
+import numpy as np
+
+from cases import make_image, split_kwargs, sweep_case_id, sweep_config
 
 # name, image kind, H, W, K, kwargs (split_kwargs: max_iter, compactness, min_size_factor, subsample_stride,
 # convert_to_lab, sigma).  Shapes with W % 8 != 0 are among them; S = (int)sqrt(H W / K).
@@ -25,6 +27,15 @@ LSC_CASES = [
 LSC_NAN_CASES = ("S1_20x20_K300", "S3_60x84_K500")
 # GPU suite only (the CPU checker is slow on it; it is the bench's image shape)
 LSC_BIG_CASE = ("hd_720x1280_K1600", "syn", 720, 1280, 1600, {})
+
+
+def lsc_sweep_case(seed):
+    """Seeded random LSC case (tests/cases.py::sweep_config) in the form of LSC_CASES."""
+    kind, H, W, K, kw = sweep_config(np.random.RandomState(17000 + seed), seed)
+    return ("sweep%d_%s" % (seed, sweep_case_id((kind, H, W, K, kw))), kind, H, W, K, kw)
+
+
+LSC_SWEEP_CASES = [lsc_sweep_case(seed) for seed in range(16)]
 
 
 def lsc_args(a):
@@ -52,5 +63,5 @@ def lsc_outputs(impl, case, stages=("means", "weights", "cinit", "cfinal"), **kw
 def lsc_reference_outputs(impl):
     """Every (key prefix, {name: array}) of tests/golden/lsc_reference_digests.npz, computed by the compiled reference
     `impl` (oracle_lsc.lsc.Ref) with num_threads = 1."""
-    for case in LSC_CASES:
+    for case in LSC_CASES + LSC_SWEEP_CASES:
         yield "lsc/" + case[0], lsc_outputs(impl, case, num_threads=1)

@@ -10,9 +10,10 @@ import sys
 import numpy as np
 import pytest
 
-from cases import (EDGE_CASES, PIPELINE_CASES, REF_ARCHS, REF_GRAPH_CASES, REF_PREEMPT_CASES, REF_REAL_CASES,
-                   big_init_outputs, digest, gpu_suite_cases, graph_outputs, make_image, pipeline_outputs,
-                   preemptive_outputs, random_config_case, real_dist_outputs, split_kwargs)
+from cases import (EDGE_CASES, K_MAX, PIPELINE_CASES, PREEMPT_SWEEP_SEEDS, REAL_SWEEP_SEEDS, REF_ARCHS, REF_GRAPH_CASES,
+                   REF_PREEMPT_CASES, REF_REAL_CASES, SWEEP_REGIONS, big_init_outputs, digest, gpu_suite_cases,
+                   graph_outputs, make_image, pipeline_outputs, preempt_sweep_case, preemptive_outputs,
+                   random_config_case, real_dist_outputs, real_sweep_case, split_kwargs, sweep_regions, sweep_S)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "golden_v1.npz")
@@ -116,6 +117,25 @@ def test_oracle_matches_compiled_reference_gpu_suite_cases(port, ref_sha, prefix
     restatement reproduces the compiled reference's outputs there, so the GPU suite compares with the reference even
     where oracle/_ref is not built."""
     _check_ref(ref_sha, prefix, fn(port))
+
+
+def test_sweeps_reach_the_regions_the_case_lists_leave_out():
+    """Every seeded sweep of the float-distance, preemptive, Euclidean and LSC contexts has at least one case in each
+    region of SWEEP_REGIONS (S <= 2, S > 110, K > 4096, one row or column, stride 1 and >= 5, max_iter 0, Lab off,
+    min_size_factor >= 1, a flat image, ...): a change of the generator that drops one fails here."""
+    from euclid_cases import EUCLID_PREEMPT_SWEEP, EUCLID_REAL_SWEEP
+    from lsc_cases import LSC_SWEEP_CASES
+    sweeps = {"float-distance": [real_sweep_case(s)[0] for s in REAL_SWEEP_SEEDS],
+              "preemptive": [preempt_sweep_case(s) for s in PREEMPT_SWEEP_SEEDS],
+              "Euclidean float-distance": [c for c, _ in EUCLID_REAL_SWEEP],
+              "Euclidean preemptive": EUCLID_PREEMPT_SWEEP, "LSC": [c[1:] for c in LSC_SWEEP_CASES]}
+    for name, cases in sweeps.items():
+        reached = set().union(*[sweep_regions(c) for c in cases])
+        assert not set(SWEEP_REGIONS) - reached, (name, sorted(set(SWEEP_REGIONS) - reached))
+        for c in cases:  # only configurations the product accepts: S >= 1, K below the u16 label limit
+            assert 1 <= c[3] <= min(K_MAX, c[1] * c[2]) and sweep_S(*c[1:4]) >= 1, (name, c)
+    assert {v for _, v in (real_sweep_case(s) for s in REAL_SWEEP_SEEDS)} == {0, 1, 2}
+    assert {v for _, v in EUCLID_REAL_SWEEP} == {0, 2}
 
 
 def test_reference_thread_and_arch_invariance(port, ref_sha):

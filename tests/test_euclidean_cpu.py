@@ -7,9 +7,10 @@ import numpy as np
 import pytest
 
 from cases import digest
-from euclid_cases import (EUCLID_ARCHS, EUCLID_CASES, EUCLID_L2_CASES, EUCLID_PREEMPT_CASES, EUCLID_REAL_CASES,
-                          EUCLID_SAME_CASES, EUCLID_WARM_CASE, case_id, euclid_pipeline_outputs, euclid_preempt_outputs, euclid_real_outputs,
-                          preempt_case_id, real_case_id)
+from euclid_cases import (EUCLID_ARCHS, EUCLID_CASES, EUCLID_L2_CASES, EUCLID_PREEMPT_CASES, EUCLID_PREEMPT_SWEEP,
+                          EUCLID_REAL_CASES, EUCLID_REAL_SWEEP, EUCLID_SAME_CASES, EUCLID_WARM_CASE, case_id,
+                          euclid_pipeline_outputs, euclid_preempt_outputs, euclid_real_outputs, preempt_case_id,
+                          preempt_sweep_id, real_case_id, real_sweep_id)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF_DIGESTS = os.path.join(ROOT, "tests", "golden", "euclid_reference_digests.npz")
@@ -82,6 +83,20 @@ def test_oracle_euclidean_real_dist_matches_compiled_reference(eport, port, ref_
     got = euclid_real_outputs(eport, variant, case)
     _check_ref(ref_sha, "euclid/" + real_case_id(variant, case), got)
     assert _differs(got, euclid_real_outputs(port, variant, case)), "the case does not exercise the option"
+
+
+@pytest.mark.parametrize("seed", range(len(EUCLID_REAL_SWEEP)))
+def test_oracle_euclidean_real_dist_sweep_matches_compiled_reference(eport, ref_sha, seed):
+    """The seeded sweep of SlicRealDist / SlicRealDistNoQ with the flag off (tests/cases.py::sweep_config), cold and warm."""
+    case, variant = EUCLID_REAL_SWEEP[seed]
+    _check_ref(ref_sha, "euclid/" + real_sweep_id(seed), euclid_real_outputs(eport, variant, case))
+
+
+@pytest.mark.parametrize("seed", range(len(EUCLID_PREEMPT_SWEEP)))
+def test_oracle_euclidean_preemptive_sweep_matches_compiled_reference(eport, ref_sha, seed):
+    got = euclid_preempt_outputs(eport, EUCLID_PREEMPT_SWEEP[seed])
+    for top in ARCH_PREFIXES:
+        _check_ref(ref_sha, "%s/%s" % (top, preempt_sweep_id(seed)), got)
 
 
 def test_oracle_l2_variant_ignores_the_flag(port, eport, ref_sha):

@@ -5,9 +5,10 @@ import numpy as np
 import pytest
 import torch
 
-from cases import make_image, split_kwargs
-from euclid_cases import (EUCLID_CASES, EUCLID_PREEMPT_CASES, EUCLID_REAL_CASES, EUCLID_SAME_CASES, EUCLID_WARM_CASE,
-                          case_id, preempt_case_id)
+from cases import make_image, split_kwargs, sweep_case_id
+from euclid_cases import (EUCLID_CASES, EUCLID_PREEMPT_CASES, EUCLID_PREEMPT_SWEEP, EUCLID_REAL_CASES, EUCLID_REAL_SWEEP,
+                          EUCLID_SAME_CASES, EUCLID_WARM_CASE, case_id, preempt_case_id, preempt_sweep_id)
+from class_checks import PREEMPT, check_class_call
 
 pytestmark = pytest.mark.gpu
 
@@ -38,9 +39,9 @@ class Euclid:
                                   stages=stages, preemptive=preemptive, preemptive_thres=preemptive_thres, **self._kw)
 
     def iterate_real(self, variant, image, clusters, max_iter=10, compactness=10.0, min_size_factor=0.25, stride=3,
-                     convert_to_lab=True):
+                     convert_to_lab=True, stages=False):
         return self._impl.iterate_real(variant, image, clusters, max_iter, compactness, min_size_factor, stride,
-                                       convert_to_lab)
+                                       convert_to_lab, stages=stages)
 
 
 @pytest.fixture(scope="module")
@@ -141,11 +142,18 @@ def test_euclidean_ldg_kernel_forced(euclid, monkeypatch, group, case, seed):
         clear_engine_cache()
 
 
-@pytest.mark.parametrize("variant", ["standard", "l2", "noq"])
-@pytest.mark.parametrize("case", EUCLID_REAL_CASES, ids=lambda c: "%s_%dx%d_K%d" % c[:4])
+VARIANTS = ("standard", "l2", "noq")
+# the hand-picked cases under every variant, then the seeded sweep (variants 0 and 2 by seed)
+REAL_PARAMS = [(v, c) for c in EUCLID_REAL_CASES for v in VARIANTS] + [(VARIANTS[v], c) for c, v in EUCLID_REAL_SWEEP]
+REAL_IDS = ["%s_%dx%d_K%d-%s" % (c[:4] + (v,)) for c in EUCLID_REAL_CASES for v in VARIANTS] + \
+           ["sweep%d_%s-%s" % (s, sweep_case_id(c), VARIANTS[v]) for s, (c, v) in enumerate(EUCLID_REAL_SWEEP)]
+
+
+@pytest.mark.parametrize("variant,case", REAL_PARAMS, ids=REAL_IDS)
 def test_euclidean_real_dist(euclid, variant, case):
     """SlicRealDist (coef * hypot, untruncated) and SlicRealDistNoQ (squared differences) with the flag off, cold and
-    warm start; SlicRealDistL2 ignores the flag, as the reference does."""
+    warm start: labels, pre-CCA labels, Cluster bytes and the variant's kernel; SlicRealDistL2 ignores the flag, as the
+    reference does."""
     import fast_slic_b200 as fs
     kind, H, W, K, kw = case
     sigma, a = split_kwargs(kw)
@@ -155,20 +163,26 @@ def test_euclidean_real_dist(euclid, variant, case):
                                  subsample_stride=a["subsample_stride"], convert_to_lab=a["convert_to_lab"],
                                  manhattan_spatial_dist=manhattan)
     s, plain = make(False), make(True)
-    v = {"standard": 0, "l2": 1, "noq": 2}[variant]
+    v = VARIANTS.index(variant)
     cl = euclid.initialize(img, K)
     for round_ in range(2):
         got = s.iterate(img, a["max_iter"]).view(np.uint16)
-        want = euclid.iterate_real(v, img, cl, *_args(a))
-        assert (got == want).all(), "%s round %d: %d px differ" % (variant, round_, int((got != want).sum()))
-        assert s.slic_model.cluster_array.tobytes() == cl.tobytes(), "%s round %d: Cluster bytes" % (variant, round_)
+        want, want_pre = euclid.iterate_real(v, img, cl, *_args(a), stages=True)
+        check_class_call("%s round %d" % (variant, round_), s, got, want, want_pre, cl, 10 + v, a["max_iter"])
         if v == 1:
             assert (plain.iterate(img, a["max_iter"]).view(np.uint16) == got).all()
             assert plain.slic_model.cluster_array.tobytes() == cl.tobytes()
 
 
-@pytest.mark.parametrize("case", EUCLID_PREEMPT_CASES, ids=[preempt_case_id(c) for c in EUCLID_PREEMPT_CASES])
+PREEMPT_PARAMS = EUCLID_PREEMPT_CASES + EUCLID_PREEMPT_SWEEP
+PREEMPT_IDS = [preempt_case_id(c) for c in EUCLID_PREEMPT_CASES] + \
+              ["%s_%s_t%g" % (preempt_sweep_id(s), sweep_case_id(c), c[4]) for s, c in enumerate(EUCLID_PREEMPT_SWEEP)]
+
+
+@pytest.mark.parametrize("case", PREEMPT_PARAMS, ids=PREEMPT_IDS)
 def test_euclidean_preemptive(euclid, case):
+    """Slic(preemptive=True, manhattan_spatial_dist=False), cold and warm start: labels, pre-CCA labels, Cluster bytes
+    and k_assign_preempt on the update passes."""
     import fast_slic_b200 as fs
     kind, H, W, K, thres, kw = case
     sigma, a = split_kwargs(kw)
@@ -179,9 +193,8 @@ def test_euclidean_preemptive(euclid, case):
     cl = euclid.initialize(img, K)
     for round_ in range(2):
         got = s.iterate(img, a["max_iter"]).view(np.uint16)
-        want = euclid.iterate(img, cl, *_args(a), preemptive=True, preemptive_thres=thres)
-        assert (got == want).all(), "round %d: %d px differ" % (round_, int((got != want).sum()))
-        assert s.slic_model.cluster_array.tobytes() == cl.tobytes(), "round %d: Cluster bytes" % round_
+        want, _, want_pre = euclid.iterate(img, cl, *_args(a), stages=True, preemptive=True, preemptive_thres=thres)
+        check_class_call("round %d" % round_, s, got, want, want_pre, cl, PREEMPT, a["max_iter"])
 
 
 def test_euclidean_iterate_batch(euclid):

@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 
 from cases import digest
-from lsc_cases import LSC_CASES, LSC_NAN_CASES, lsc_args, lsc_image, lsc_outputs
+from lsc_cases import LSC_CASES, LSC_NAN_CASES, LSC_SWEEP_CASES, lsc_args, lsc_image, lsc_outputs
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF_DIGESTS = os.path.join(ROOT, "tests", "golden", "lsc_reference_digests.npz")
@@ -24,7 +24,7 @@ def ref_sha():
     return {k: bytes(v) for k, v in zip(z["keys"].tolist(), z["sha"])}
 
 
-@pytest.mark.parametrize("case", LSC_CASES, ids=[c[0] for c in LSC_CASES])
+@pytest.mark.parametrize("case", LSC_CASES + LSC_SWEEP_CASES, ids=[c[0] for c in LSC_CASES + LSC_SWEEP_CASES])
 def test_oracle_lsc_matches_compiled_reference(lport, ref_sha, case):
     """Initial clusters, pre-CCA and final labels, Cluster bytes, feature means, pixel weights and the centroid
     features after before_iteration and at the end equal the reference's ContextLSC with num_threads=1, cold and warm."""
@@ -42,6 +42,13 @@ def test_cases_reach_the_empty_cluster_path(lport):
         out = lsc_outputs(lport, case)
         nan = any(np.isnan(out["cfinal%d" % r]).any() for r in (0, 1))
         assert nan == (case[0] in LSC_NAN_CASES), case[0]
+
+
+def test_sweep_reaches_the_empty_cluster_path(lport):
+    """The seeded LSC sweep has cases that leave NaN centroid features and cases that do not."""
+    nan = [any(np.isnan(out["cfinal%d" % r]).any() for r in (0, 1))
+           for out in (lsc_outputs(lport, case) for case in LSC_SWEEP_CASES)]
+    assert any(nan) and not all(nan), nan
 
 
 def test_reference_with_four_threads_changes_the_centroids():

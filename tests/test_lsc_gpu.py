@@ -5,7 +5,8 @@ import numpy as np
 import pytest
 import torch
 
-from lsc_cases import LSC_BIG_CASE, LSC_CASES, lsc_args, lsc_image
+from class_checks import LSC, assert_kernel
+from lsc_cases import LSC_BIG_CASE, LSC_CASES, LSC_SWEEP_CASES, lsc_args, lsc_image
 
 pytestmark = pytest.mark.gpu
 
@@ -49,10 +50,16 @@ def _compare(lsc_checker, case, manhattan=True):
         assert (lab == want).all(), "%s round %d: labels differ (%d px)" % (name, r, int((lab != want).sum()))
         assert cl_gpu[0].cpu().numpy().tobytes() == cl.tobytes(), "%s round %d: Cluster bytes differ" % (name, r)
         _stages_equal(name, r, eng, st)
+        assert_kernel("%s round %d" % (name, r), eng.dispatch(), LSC, a["max_iter"])
 
 
-@pytest.mark.parametrize("case", LSC_CASES + [LSC_BIG_CASE], ids=[c[0] for c in LSC_CASES + [LSC_BIG_CASE]])
+ENGINE_CASES = LSC_CASES + [LSC_BIG_CASE] + LSC_SWEEP_CASES
+
+
+@pytest.mark.parametrize("case", ENGINE_CASES, ids=[c[0] for c in ENGINE_CASES])
 def test_lsc_engine_matches_checker(lsc_checker, case):
+    """The hand-picked cases, the bench's shape and the seeded sweep (lsc_cases.py::lsc_sweep_case): every stage of both
+    calls, on k_assign_lsc."""
     _compare(lsc_checker, case)
 
 

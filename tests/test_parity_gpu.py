@@ -7,8 +7,10 @@ import numpy as np
 import pytest
 import torch
 
-from cases import (BIG_CASES, EDGE_CASES, LDG_FORCED_CASES, PIPELINE_CASES, TMA_CASES, cca_random_labels, cca_range_labels,
-                   gpu_random_config_case, make_image, split_kwargs)
+from cases import (BIG_CASES, EDGE_CASES, LDG_FORCED_CASES, PIPELINE_CASES, PREEMPT_SWEEP_SEEDS, REAL_SWEEP_SEEDS,
+                   SWEEP_KINDS, TMA_CASES, cca_random_labels, cca_range_labels, gpu_random_config_case, make_image,
+                   preempt_sweep_case, real_sweep_case, split_kwargs, sweep_case_id)
+from class_checks import LSC, PREEMPT, REAL_KERNELS, assert_kernel, check_class_call
 
 pytestmark = pytest.mark.gpu
 
@@ -496,12 +498,21 @@ REAL_CASES = [("syn", 120, 160, 48, {}), ("noise", 97, 131, 37, dict(min_size_fa
               ("thin", 10, 400, 5, {})]
 
 
-@pytest.mark.parametrize("variant", ["standard", "l2", "noq"])
-@pytest.mark.parametrize("case", REAL_CASES, ids=lambda c: "%s_%dx%d_K%d" % c[:4])
+REAL_VARIANTS = ("standard", "l2", "noq")
+
+# the hand-picked cases under every variant, then the seeded sweep (tests/cases.py::real_sweep_case), variant by seed
+REAL_SWEEP = [(REAL_VARIANTS[v], c) for c, v in (real_sweep_case(s) for s in REAL_SWEEP_SEEDS)]
+REAL_PARAMS = [(v, c) for c in REAL_CASES for v in REAL_VARIANTS] + REAL_SWEEP
+REAL_IDS = ["%s_%dx%d_K%d-%s" % (c[:4] + (v,)) for c in REAL_CASES for v in REAL_VARIANTS] + \
+           ["sweep%d_%s-%s" % (s, sweep_case_id(c), v) for s, (v, c) in enumerate(REAL_SWEEP)]
+
+
+@pytest.mark.parametrize("variant,case", REAL_PARAMS, ids=REAL_IDS)
 def test_real_dist_variants(checker, variant, case):
     """SlicRealDist / SlicRealDistL2 / SlicRealDistNoQ (fast_slic/base_slic.py:64-85 -> context.cpp:394-499) on the GPU:
-    float distances, every operation in the reference's order and rounding -- labels and raw Cluster bytes (float
-    centroids of the NoQ variant included) identical to the compiled reference, cold start and warm start."""
+    float distances, every operation in the reference's order and rounding -- labels, pre-CCA labels and raw Cluster
+    bytes (float centroids of the NoQ variant included) identical to the compiled reference, cold start and warm start,
+    on k_assign_real of the variant."""
     import fast_slic_b200 as fs
     kind, H, W, K, kw = case
     kind = "syn" if kind == "thin" else kind
@@ -510,16 +521,14 @@ def test_real_dist_variants(checker, variant, case):
     cls = {"standard": fs.SlicRealDist, "l2": fs.SlicRealDistL2, "noq": fs.SlicRealDistNoQ}[variant]
     s = cls(num_components=K, compactness=args["compactness"], min_size_factor=args["min_size_factor"],
             subsample_stride=args["subsample_stride"], convert_to_lab=args["convert_to_lab"])
-    v = {"standard": 0, "l2": 1, "noq": 2}[variant]
+    v = REAL_VARIANTS.index(variant)
     cl = checker.initialize(img, K)
     for round_ in range(2):
         got = s.iterate(img, args["max_iter"]).view(np.uint16)
-        want = checker.iterate_real(v, img, cl, args["max_iter"], args["compactness"], args["min_size_factor"],
-                                    args["subsample_stride"], args["convert_to_lab"])
-        assert (got == want).all(), "%s round %d: %d px differ" % (variant, round_, int((got != want).sum()))
-        gc = s.slic_model.cluster_array
-        for f in ("y", "x", "r", "g", "b", "num_members", "number", "is_active", "is_updatable"):
-            assert (gc[f] == cl[f]).all(), "%s round %d: cluster field %s" % (variant, round_, f)
+        want, want_pre = checker.iterate_real(v, img, cl, args["max_iter"], args["compactness"], args["min_size_factor"],
+                                              args["subsample_stride"], args["convert_to_lab"], stages=True)
+        check_class_call("%s round %d" % (variant, round_), s, got, want, want_pre, cl, REAL_KERNELS[variant],
+                          args["max_iter"])
 
 
 PREEMPT_CASES = [("syn", 120, 160, 48, 0.05, {}), ("syn", 200, 300, 150, 0.05, {}), ("syn", 240, 320, 200, 0.2, dict(max_iter=15)),
@@ -528,12 +537,18 @@ PREEMPT_CASES = [("syn", 120, 160, 48, 0.05, {}), ("syn", 200, 300, 150, 0.05, {
                  ("syn", 480, 640, 400, 0.05, dict(sigma=4.0)), ("syn", 720, 1280, 1600, 0.05, dict(min_size_factor=0.0))]
 
 
-@pytest.mark.parametrize("case", PREEMPT_CASES, ids=lambda c: "%s_%dx%d_K%d_t%g" % c[:5])
+PREEMPT_SWEEP = [preempt_sweep_case(s) for s in PREEMPT_SWEEP_SEEDS]
+PREEMPT_IDS = ["%s_%dx%d_K%d_t%g" % c[:5] for c in PREEMPT_CASES] + \
+              ["sweep%d_%s_t%g" % (s, sweep_case_id(c), c[4]) for s, c in enumerate(PREEMPT_SWEEP)]
+
+
+@pytest.mark.parametrize("case", PREEMPT_CASES + PREEMPT_SWEEP, ids=PREEMPT_IDS)
 def test_preemptive(checker, case):
     """Slic(preemptive=True, preemptive_thres=t) (fast_slic/base_slic.py:12-13 -> preemptive.h, context.cpp:218,307-385):
-    clusters that stopped moving drop out of assign and update.  Labels and the raw Cluster records -- including the
-    is_updatable countdown the reference leaves in them -- identical to the compiled reference, cold and warm start; the
-    option really bites (the result differs from the non-preemptive one)."""
+    clusters that stopped moving drop out of assign and update.  Labels, pre-CCA labels and the raw Cluster records --
+    including the is_updatable countdown the reference leaves in them -- identical to the compiled reference, cold and
+    warm start, with k_assign_preempt on the update passes; on the hand-picked cases the option really bites (the result
+    differs from the non-preemptive one), the seeded sweep (tests/cases.py::preempt_sweep_case) is parity only."""
     import fast_slic_b200 as fs
     kind, H, W, K, thres, kw = case
     sigma, args = split_kwargs(kw)
@@ -546,13 +561,11 @@ def test_preemptive(checker, case):
                             args["subsample_stride"], args["convert_to_lab"])
     for round_ in range(2):
         got = s.iterate(img, args["max_iter"]).view(np.uint16)
-        want = checker.iterate(img, cl, args["max_iter"], args["compactness"], args["min_size_factor"], args["subsample_stride"],
-                               args["convert_to_lab"], preemptive=True, preemptive_thres=thres)
-        assert (got == want).all(), "round %d: %d px differ" % (round_, int((got != want).sum()))
-        gc = s.slic_model.cluster_array
-        for f in ("y", "x", "r", "g", "b", "num_members", "number", "is_active", "is_updatable"):
-            assert (gc[f] == cl[f]).all(), "round %d: cluster field %s" % (round_, f)
-        if round_ == 0 and kind != "noise":
+        want, _, want_pre = checker.iterate(img, cl, args["max_iter"], args["compactness"], args["min_size_factor"],
+                                            args["subsample_stride"], args["convert_to_lab"], stages=True, preemptive=True,
+                                            preemptive_thres=thres)
+        check_class_call("round %d" % round_, s, got, want, want_pre, cl, PREEMPT, args["max_iter"])
+        if round_ == 0 and kind != "noise" and case in PREEMPT_CASES:
             assert (want != plain).any(), "the case does not exercise the option"
 
 
@@ -591,23 +604,98 @@ def test_random_configurations(checker, seed):
     _compare(name + " warm", _run_cuda(img, K, args, iterate_twice=True), _run_oracle(checker, img, K, args, iterate_twice=True))
 
 
-def test_iterate_batch_variants(checker):
-    """iterate_batch() of the float-distance classes and of Slic(preemptive=True): every image of a host batch and of a
-    device batch equals the single-image result of the compiled reference (the batch entry must not fall back to the
-    default integer path)."""
+@pytest.fixture(scope="module")
+def sweep_checkers(checker):
+    """(Euclidean checker, its extra iterate keyword arguments, LSC checker), chosen as test_euclidean_gpu.py and
+    test_lsc_gpu.py choose them: the compiled reference where it was built, else the restatement."""
+    from oracle_euclid.euclid import Port as EPort, Ref as ERef
+    from oracle_lsc.lsc import Port as LPort, Ref as LRef
+    ekw = dict(arch="x64/avx2", num_threads=checker._threads) if ERef.available() else {}
+    return ERef() if ERef.available() else EPort(), ekw, LRef() if LRef.available() else LPort()
+
+
+def _batch_specs():
+    """(family, float-distance variant, case (kind, H, W, K, [thres,] kwargs), image kinds, image seed) per input of
+    test_iterate_batch_variants: the original three classes on one shape, then every fourth seed of each sweep with three
+    images of different kinds."""
+    from euclid_cases import EUCLID_PREEMPT_SWEEP, EUCLID_REAL_SWEEP
+    from lsc_cases import LSC_SWEEP_CASES
+    base, kinds = ("syn", 120, 160, 48, {}), ("syn", "blocks", "syn")
+    specs = [("l2", ("real", 1, base, kinds, 610)), ("noq", ("real", 2, base, kinds, 610)),
+             ("preemptive", ("preemptive", None, base[:4] + (0.1, {}), kinds, 610))]
+    sweeps = [("real", [(v, c) for c, v in (real_sweep_case(s) for s in REAL_SWEEP_SEEDS)]),
+              ("preemptive", [(None, c) for c in PREEMPT_SWEEP]),
+              ("euclid_real", [(v, c) for c, v in EUCLID_REAL_SWEEP]),
+              ("euclid_preemptive", [(None, c) for c in EUCLID_PREEMPT_SWEEP]),
+              ("lsc", [(None, c[1:]) for c in LSC_SWEEP_CASES])]
+    for family, cases in sweeps:
+        for seed in range(0, len(cases), 4):
+            v, c = cases[seed]
+            three = (c[0],) + tuple(k for k in SWEEP_KINDS if k != c[0])[:2]
+            specs.append(("%s_sweep%d%s" % (family, seed, "" if v is None else "_v%d" % v),
+                          (family, v, c, three, 620 + seed)))
+    return specs
+
+
+BATCH_SPECS = _batch_specs()
+
+
+def test_iterate_batch_variants(checker, sweep_checkers):
+    """iterate_batch() of the float-distance classes, of Slic(preemptive=True), of both with manhattan_spatial_dist=False
+    and of LSC(num_threads=1), on every input of BATCH_SPECS: every image of a host batch and of a device batch equals the
+    single-image result of the checker -- labels, pre-CCA labels, Cluster bytes -- and the batch entry ran the class's
+    kernel (it must not fall back to the default integer path).  Every input runs; the failure names all that failed."""
+    failed = []
+    for name, spec in BATCH_SPECS:
+        try:
+            _check_batch(checker, sweep_checkers, spec)
+        except AssertionError as e:
+            failed.append("%s: %s" % (name, (str(e).splitlines() or ["assertion failed"])[0]))
+    assert not failed, "%d of %d inputs differ:\n%s" % (len(failed), len(BATCH_SPECS), "\n".join(failed))
+
+
+def _check_batch(checker, sweep_checkers, spec):
     import fast_slic_b200 as fs
-    H, W, K, B = 120, 160, 48, 3
-    imgs = np.stack([make_image("syn" if b != 1 else "blocks", H, W, seed=610 + b) for b in range(B)])
-    for name, obj, ref_call in (
-            ("l2", fs.SlicRealDistL2(num_components=K), lambda im, cl: checker.iterate_real(1, im, cl, 10, 10.0, 0.25, 3, True)),
-            ("noq", fs.SlicRealDistNoQ(num_components=K), lambda im, cl: checker.iterate_real(2, im, cl, 10, 10.0, 0.25, 3, True)),
-            ("preemptive", fs.Slic(num_components=K, preemptive=True, preemptive_thres=0.1),
-             lambda im, cl: checker.iterate(im, cl, 10, 10.0, 0.25, 3, True, preemptive=True, preemptive_thres=0.1))):
-        lab_h, cl_h = obj.iterate_batch(imgs, return_clusters=True)
-        lab_d, cl_d = obj.iterate_batch(torch.from_numpy(imgs).cuda(), return_clusters=True)
-        for b in range(B):
-            cl = checker.initialize(imgs[b], K)
-            want = ref_call(imgs[b], cl)
-            assert (lab_h[b].view(np.uint16) == want).all(), (name, "host", b)
-            assert (lab_d[b].cpu().numpy().view(np.uint16) == want).all(), (name, "device", b)
-            assert cl_h[b].tobytes() == cl.tobytes() == cl_d[b].cpu().numpy().tobytes(), (name, b)
+    from fast_slic_b200 import get_engine
+    family, v, case, kinds, img_seed = spec
+    euclid, ekw, lsc_checker = sweep_checkers
+    kind, H, W, K = case[:4]
+    thres = case[4] if len(case) == 6 else None
+    sigma, a = split_kwargs(case[-1])
+    args = (a["max_iter"], a["compactness"], a["min_size_factor"], a["subsample_stride"], a["convert_to_lab"])
+    B = len(kinds)
+    imgs = np.stack([make_image(k, H, W, seed=img_seed + b, sigma=sigma) for b, k in enumerate(kinds)])
+    real_cls = (fs.SlicRealDist, fs.SlicRealDistL2, fs.SlicRealDistNoQ)
+    cls, ckw, kernel, run = {
+        "real": (real_cls[v or 0], {}, 10 + (v or 0),
+                 lambda im, cl: checker.iterate_real(v, im, cl, *args, stages=True)),
+        "preemptive": (fs.Slic, dict(preemptive=True, preemptive_thres=thres), PREEMPT,
+                       lambda im, cl: checker.iterate(im, cl, *args, stages=True, preemptive=True,
+                                                      preemptive_thres=thres)[::2]),
+        "euclid_real": (real_cls[v or 0], dict(manhattan_spatial_dist=False), 10 + (v or 0),
+                        lambda im, cl: euclid.iterate_real(v, im, cl, *args, stages=True)),
+        "euclid_preemptive": (fs.Slic, dict(preemptive=True, preemptive_thres=thres, manhattan_spatial_dist=False), PREEMPT,
+                              lambda im, cl: euclid.iterate(im, cl, *args, stages=True, preemptive=True,
+                                                            preemptive_thres=thres, **ekw)[::2]),
+        "lsc": (fs.LSC, dict(num_threads=1), LSC,
+                lambda im, cl: (lambda lab, st: (lab, st["pre"]))(*lsc_checker.iterate_lsc(im, cl, *args, stages=True))),
+    }[family]
+    obj = cls(num_components=K, compactness=a["compactness"], min_size_factor=a["min_size_factor"],
+              subsample_stride=a["subsample_stride"], convert_to_lab=a["convert_to_lab"], **ckw)
+    want = []
+    for b in range(B):
+        cl = checker.initialize(imgs[b], K)
+        lab, pre = run(imgs[b], cl)
+        want.append((lab, pre, cl.tobytes()))
+    for where, src in (("host", imgs), ("device", torch.from_numpy(imgs).cuda())):
+        lab, cl = obj.iterate_batch(src, max_iter=a["max_iter"], return_clusters=True)
+        eng = get_engine(H, W, K, B)
+        pre = eng.debug_stages(B)[1].cpu().numpy().view(np.uint16)
+        assert_kernel("%s %s" % (family, where), eng.dispatch(), kernel, a["max_iter"])
+        if where == "device":
+            lab, cl = lab.cpu().numpy(), cl.cpu().numpy()
+        for b, (wlab, wpre, wcl) in enumerate(want):
+            name = "%s %s image %d (%s)" % (family, where, b, kinds[b])
+            assert (pre[b] == wpre).all(), "%s: pre-CCA labels differ (%d px)" % (name, int((pre[b] != wpre).sum()))
+            assert (lab[b].view(np.uint16) == wlab).all(), "%s: labels differ" % name
+            assert cl[b].tobytes() == wcl, "%s: Cluster bytes differ" % name
