@@ -87,14 +87,16 @@ struct fslic_ctx {
     // cca state (sized for cca_batch images at a time)
     int cca_batch = 1;
     int* par = nullptr;            // [Bc][N]
-    uint32_t* aux = nullptr;       // [Bc][N]  area at root pixel, then component number
-    int* cleader = nullptr;        // [Bc][N]
-    uint32_t* carea = nullptr;     // [Bc][N]
-    uint16_t* cnew = nullptr;      // [Bc][N]
-    uint16_t* fin = nullptr;       // [Bc][N]  (second half of the cnew allocation)
+    uint32_t* aux = nullptr;       // [Bc][N]  area at root pixel
+    uint32_t* carea = nullptr;     // [Bc][N]  area by component number
+    uint16_t* cnew = nullptr;      // [Bc][N]  new label by component number
+    uint16_t* fin = nullptr;       // [Bc][N]  final label at root pixel (second half of the cnew allocation)
     int* rootbuf = nullptr;        // [Bc][N] ordered root lists of k_ccl_flatten
-    int* blkcnt = nullptr;         // [Bc][nblk]
-    int* blkoff = nullptr;         // [Bc][nblk]
+    int* predbuf = nullptr;        // [Bc][N] predecessor root of every rootbuf entry
+    unsigned long long* chunkinfo = nullptr;  // [Bc][nblk * 32] root mask and root-list offset of every 32-pixel chunk
+    int* blkcnt = nullptr;         // [Bc][nblk] roots per block, then kept components per 1024-component chunk
+    int* blkoff = nullptr;         // [Bc][nblk] component number of the first root of a block
+    int* kblkoff = nullptr;        // [Bc][nblk] kept components in front of a 1024-component chunk
     CcaCounters* counters = nullptr;  // [Bc]
     unsigned int* ahist = nullptr;    // [Bc][CCA_HIST] histogram of candidate areas
     unsigned long long* heap = nullptr;  // [Bc][Kheap]
@@ -250,8 +252,8 @@ extern "C" int fslic_b200_destroy(fslic_ctx* c) {
     if (!c) return FSLIC_OK;
     DeviceGuard dev_guard__(c->device);
     void* ptrs[] = {c->d_gamma, c->d_labtbl, c->quad,   c->labels,  c->cinfo,  c->acc,    c->cell_start,
-                    c->cinfo_tmp, c->cell_cnt, c->prep_tickets, c->sptable, c->par,  c->aux,    c->cleader, c->carea,
-                    c->cnew,    c->rootbuf, c->blkcnt, c->blkoff,  c->counters, c->ahist, c->heap, c->d_img,
+                    c->cinfo_tmp, c->cell_cnt, c->prep_tickets, c->sptable, c->par,  c->aux,    c->predbuf, c->carea,
+                    c->cnew,    c->chunkinfo, c->rootbuf, c->blkcnt, c->blkoff,  c->kblkoff, c->counters, c->ahist, c->heap, c->d_img,
                     c->d_cl,    c->d_lab};
     for (void* p : ptrs)
         if (p) cudaFree(p);
@@ -349,7 +351,7 @@ static int create_impl(int device, int H, int W, int K, int max_batch, bool cca_
         CKC(dalloc(&c->sptable, (size_t)2 * SPT_MAX_ELEMS));
     }
 
-    // CCA scratch: 26 B/pixel/image; cap the resident set at an eighth of the device's memory (10 GB on an 80 GB H100,
+    // CCA scratch: 26 B/pixel/image (24.25 used); cap the resident set at an eighth of the device's memory (10 GB on an 80 GB H100,
     // so that several contexts per GPU fit beside their assign state) and at most 12 GB; larger batches run the
     // connectivity stage in sub-batches
     const size_t per_img = N * 26 + 4096;
@@ -367,13 +369,15 @@ static int create_impl(int device, int H, int W, int K, int max_batch, bool cca_
     const int nblk = ceil_div(c->N, CCA_BLOCK);
     CKC(dalloc(&c->par, bc * N));
     CKC(dalloc(&c->aux, bc * N));
-    CKC(dalloc(&c->cleader, bc * N));
     CKC(dalloc(&c->carea, bc * N));
     CKC(dalloc(&c->cnew, 2 * bc * N));
     c->fin = c->cnew + bc * N;
     CKC(dalloc(&c->rootbuf, bc * N));  // (its own array: two halves of a batch may be in different phases at the same time)
+    CKC(dalloc(&c->predbuf, bc * N));
+    CKC(dalloc(&c->chunkinfo, bc * nblk * (CCA_BLOCK / 32)));
     CKC(dalloc(&c->blkcnt, bc * nblk));
     CKC(dalloc(&c->blkoff, bc * nblk));
+    CKC(dalloc(&c->kblkoff, bc * nblk));
     CKC(dalloc(&c->counters, bc));
     CKC(cudaMemset(c->counters, 0, bc * sizeof(CcaCounters)));  // the diagnostics entry may read them before the first run
     CKC(dalloc(&c->ahist, bc * CCA_HIST));
@@ -499,13 +503,15 @@ static int run_cca(fslic_ctx* c, const uint16_t* d_in, uint16_t* d_out, int batc
     const int nblk_all = ceil_div(N, CCA_BLOCK);
     int* const x_par = c->par + so * N;
     uint32_t* const x_aux = c->aux + so * N;
-    int* const x_cleader = c->cleader + so * N;
     uint32_t* const x_carea = c->carea + so * N;
     uint16_t* const x_cnew = c->cnew + so * N;
     uint16_t* const x_fin = c->fin + so * N;
     int* const x_rootbuf = c->rootbuf + so * N;
+    int* const x_predbuf = c->predbuf + so * N;
+    unsigned long long* const x_chunkinfo = c->chunkinfo + so * nblk_all * (CCA_BLOCK / 32);
     int* const x_blkcnt = c->blkcnt + so * nblk_all;
     int* const x_blkoff = c->blkoff + so * nblk_all;
+    int* const x_kblkoff = c->kblkoff + so * nblk_all;
     CcaCounters* const x_counters = c->counters + so;
     unsigned int* const x_ahist = c->ahist + so * CCA_HIST;
     unsigned long long* const x_heap = c->heap + so * (size_t)c->heap_K;
@@ -549,7 +555,7 @@ static int run_cca(fslic_ctx* c, const uint16_t* d_in, uint16_t* d_out, int batc
             }
         }
         if (timed) CK(cudaEventRecord(c->cev[1], st));
-        k_ccl_flatten<<<g, 256, 0, st>>>(cp, in, x_par, x_aux, x_blkcnt, x_rootbuf);
+        k_ccl_flatten<<<g, 256, 0, st>>>(cp, in, x_par, x_aux, x_blkcnt, x_rootbuf, x_predbuf, x_chunkinfo);
         k_scan_blocks<<<nb, 1024, 0, st>>>(x_blkcnt, x_blkoff, cp.nblk, cp.nblk, nullptr, 0, 1,
                                            &x_counters[0].ncomp, (int)(sizeof(CcaCounters) / sizeof(int)), nullptr, -1);
         // grids of the per-component walks: sized for full batches (a few CTAs per image); a small batch gets more
@@ -559,8 +565,8 @@ static int run_cca(fslic_ctx* c, const uint16_t* d_in, uint16_t* d_out, int batc
             c->disp.cca_split = nb >= 4;
             c->disp.cca_number_nb = ceil_div(cp.nblk, number_grid * (CCA_BLOCK / 32));  // NB of k_ccl_number
         }
-        k_ccl_number<<<dim3(number_grid, nb), CCA_BLOCK, 0, st>>>(cp, x_rootbuf, x_aux, x_blkcnt, x_blkoff, x_cleader, x_carea,
-                                                                      x_counters, x_ahist);
+        k_ccl_number<<<dim3(number_grid, nb), CCA_BLOCK, 0, st>>>(cp, x_rootbuf, x_aux, x_blkcnt, x_blkoff, x_carea, x_counters,
+                                                                      x_ahist);
         if (timed) CK(cudaEventRecord(c->cev[2], st));
         k_cca_threshold<<<nb, 1024, 0, st>>>(cp, x_carea, x_counters, x_ahist);
         if (timed) CK(cudaEventRecord(c->cev[3], st));
@@ -572,18 +578,21 @@ static int run_cca(fslic_ctx* c, const uint16_t* d_in, uint16_t* d_out, int batc
         auto tail = [&](int which, cudaStream_t ts) {
             CcaParams cq = cp;
             cq.which = which;
+            // (blkoff keeps the component number of each block's first root for k_cca_absorb: the kept offsets of the
+            // 1024-component chunks go to kblkoff)
             const dim3 gk(std::min(cp.nblk, std::max(CCA_KEPT_GRID, 256 / nb)), nb);
             k_kept_count<<<gk, CCA_BLOCK, 0, ts>>>(cq, x_carea, x_counters, x_blkcnt);
-            k_scan_blocks<<<nb, 1024, 0, ts>>>(x_blkcnt, x_blkoff, cp.nblk, 0, &x_counters[0].ncomp,
+            k_scan_blocks<<<nb, 1024, 0, ts>>>(x_blkcnt, x_kblkoff, cp.nblk, 0, &x_counters[0].ncomp,
                                                (int)(sizeof(CcaCounters) / sizeof(int)), CCA_BLOCK,
                                                &x_counters[0].nkept, (int)(sizeof(CcaCounters) / sizeof(int)),
                                                x_counters, which);
-            k_kept_label<<<gk, CCA_BLOCK, 0, ts>>>(cq, x_carea, x_counters, x_blkoff, x_cnew);
-            int ab = ceil_div(N, 256 * (nb < 4 ? 2 : 8));
-            if (ab > c->num_sms * 8) ab = c->num_sms * 8;
-            dim3 ga(ab, nb);
+            k_kept_label<<<gk, CCA_BLOCK, 0, ts>>>(cq, x_carea, x_counters, x_kblkoff, x_cnew);
             if (timed) cudaEventRecord(c->cev[4], ts);
-            k_cca_absorb<<<ga, 256, 0, ts>>>(cq, x_par, x_aux, x_cleader, x_cnew, x_counters, x_fin);
+            // one warp per 1024-pixel block and its root list; below 4 images, 8 warps per block (all latency there)
+            const int nsplit = nb < 4 ? 8 : 1;
+            const dim3 ga(ceil_div(cp.nblk * nsplit, CCA_TAIL_WARPS), nb);
+            k_cca_absorb<<<ga, 32 * CCA_TAIL_WARPS, 0, ts>>>(cq, x_rootbuf, x_predbuf, x_chunkinfo, x_blkoff, x_counters,
+                                                              x_cnew, x_fin, nsplit);
             if (timed) cudaEventRecord(c->cev[5], ts);
             int ob = ceil_div(ceil_div(N, 8), 256);  // 8 pixels per thread on the vector path (any N works: grid-stride)
             if (ob > c->num_sms * 32) ob = c->num_sms * 32;
