@@ -5,8 +5,8 @@
 #include <cuda_runtime.h>
 #include "../../include/fslic_b200.h"
 
-// Stores msg as this thread's fslic_b200_last_error() and returns code.  Defined in capi.cu, next to the one
-// thread-local message every entry point of the library writes.
+// Stores msg as this thread's fslic_b200_last_error() and returns code.  Defined once, in capi.cu, next to the one
+// thread-local message that the entry points of every translation unit (capi*.cu) write.
 int set_err(int code, const std::string& msg);
 
 // Every entry point runs on the context's device and puts the caller's current device back on return

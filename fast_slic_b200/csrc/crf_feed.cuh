@@ -1,6 +1,7 @@
-// crf_feed.cuh -- the SimpleCRF's per-frame input built on the device (capi.cu's fslic_b200_crfdev_* entry points):
+// crf_feed.cuh -- the SimpleCRF's per-frame input built on the device (capi_crf.cu's fslic_b200_crfdev_* entry points):
 // cluster records, adjacency CSR and unaries, each equal bit for bit to what the host path (SimpleCRF.push_slic_frame
-// and the unary setters of fast_slic_b200/crf.py, capi.cu's fslic_b200_crf_*) stores for the same input.
+// and the unary setters of fast_slic_b200/crf.py, capi_crf.cu's fslic_b200_crf_*) stores for the same input.
+// Defines non-inline kernels: include it (and crf.cuh) from capi_crf.cu only.
 #pragma once
 #include <stdint.h>
 #include <cub/block/block_scan.cuh>

@@ -58,7 +58,7 @@ if "--one" in sys.argv:
     print("host blocking: median %.3f ms  min %.3f  p90 %.3f | device API on a stream: %.3f ms/call" % (
         1e3 * ts[100], 1e3 * ts[0], 1e3 * ts[180], e0.elapsed_time(e1) / 100))
 else:
-    for env in ({}, {"FSLIC_GRAPH": "0"}, {"FSLIC_PREPARE": "1"}, {"FSLIC_ASSIGN": "4"}, {"FSLIC_GRAPH": "0", "FSLIC_PREPARE": "1"}):
+    for env in ({}, {"FSLIC_GRAPH": "0"}, {"FSLIC_ASSIGN": "4"}):
         e = dict(os.environ)
         e.update(env)
         out = subprocess.run([sys.executable, __file__, "--one"], env=e, capture_output=True, text=True)
