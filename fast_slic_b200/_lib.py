@@ -43,6 +43,7 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_rag_batch_fill",
     "fslic_b200_gt_histogram_batch", "fslic_b200_gt_scores_scratch_bytes", "fslic_b200_gt_scores_batch",
     "fslic_b200_gt_boundaries_batch",
+    "fslic_b200_props_batch",
 )
 
 STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity", "iterate")
@@ -140,6 +141,7 @@ def lib():
     L.fslic_b200_gt_scores_batch.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, i32, i64, vp, vp, C.c_size_t,
                                              vp]
     L.fslic_b200_gt_boundaries_batch.argtypes = [i32, i32, i32, i32, vp, vp, vp]
+    L.fslic_b200_props_batch.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.fslic_b200_assign_kernel_time.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]
     L.fslic_b200_debug_cca_counters.argtypes = [vp, C.POINTER(C.c_int32), i32]
     L.fslic_b200_debug_select_profile.argtypes = [vp, C.POINTER(C.c_longlong), i32]

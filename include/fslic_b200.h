@@ -297,6 +297,24 @@ int fslic_b200_gt_scores_batch(int device, int batch, int H, int W, int K, int t
 int fslic_b200_gt_boundaries_batch(int device, int batch, int H, int W, const uint16_t* d_labels, uint8_t* d_out,
                                    void* stream);
 
+/* Superpixel shapes (props.cuh; no counterpart in the reference) of `batch` label maps d_labels u16[B,H,W]; node
+ * n = b*K + k is label k of image b, pixel (row y, column x) has coordinates (y, x).  A label outside [0, K) belongs to
+ * no superpixel.  1 <= K <= 65534, H, W <= 65535, H * W <= 2^29.  Outputs, all device memory:
+ *   d_area int32[B*K]         pixels labelled k;
+ *   d_bbox int32[B*K][4]      (y0, x0, y1, x1): min inclusive, max exclusive; all 0 for an empty node;
+ *   d_moments int64[B*K][5]   (sum y, sum x, sum y^2, sum xy, sum x^2) over k's pixels, exact;
+ *   d_perimeter int32[B*K]    sides of k's pixels whose 4-neighbour across that side is outside the image or has another
+ *                             raw label;
+ *   d_border int32[B*K]       those of the sides that lie on the image edge;
+ *   d_centroid f64[B*K][2]    (sum y / n, sum x / n);
+ *   d_covariance f64[B*K][3]  (sum y^2 / n - cy cy, sum xy / n - cy cx, sum x^2 / n - cx cx);
+ * each float64 step one correctly rounded operation, 0.0 for an empty node.  Integer arithmetic up to that, so the result
+ * of image b depends on d_labels[b] only.  No scratch; asynchronous on `stream`, never synchronises (a CUDA graph can
+ * capture it); batch == 0 does nothing, H or W == 0 zeroes the outputs. */
+int fslic_b200_props_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels, int32_t* d_area,
+                           int32_t* d_bbox, long long* d_moments, int32_t* d_perimeter, int32_t* d_border,
+                           double* d_centroid, double* d_covariance, void* stream);
+
 /* Stage probes for the parity tests (the reference's protected quad_image / assignment,
  * context.h:48-50): copies of the last iterate()'s Lab quad image [B,H,W,4] u8 and pre-CCA
  * labels [B,H,W] u16 into caller device buffers (either may be NULL). */
