@@ -15,7 +15,7 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_destroy", "fslic_b200_initialize_clusters", "fslic_b200_iterate", "fslic_b200_iterate_host",
     "fslic_b200_initialize_clusters_host", "fslic_b200_enforce_connectivity", "fslic_b200_debug_stages",
     "fslic_b200_rgb_to_quad", "fslic_b200_debug_heap_select", "fslic_b200_stage_ms", "fslic_b200_get_S",
-    "fslic_b200_launches_last_iterate", "fslic_b200_assign_kernel_time", "fslic_b200_debug_cca_counters", "fslic_b200_debug_select_profile",
+    "fslic_b200_launches_last_iterate", "fslic_b200_assign_kernel_time", "fslic_b200_debug_cca_counters",
     "fslic_b200_iterate_host_async", "fslic_b200_wait", "fslic_b200_create_cca",
     "fslic_b200_debug_assign_impl", "fslic_b200_debug_dispatch", "fslic_b200_debug_cca_dispatch", "fslic_b200_connectivity_scratch_bytes", "fslic_b200_get_connectivity",
     "fslic_b200_get_mask_density", "fslic_b200_cluster_density_to_mask", "fslic_b200_cca_stage_ms",
@@ -144,7 +144,6 @@ def lib():
     L.fslic_b200_props_batch.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.fslic_b200_assign_kernel_time.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]
     L.fslic_b200_debug_cca_counters.argtypes = [vp, C.POINTER(C.c_int32), i32]
-    L.fslic_b200_debug_select_profile.argtypes = [vp, C.POINTER(C.c_longlong), i32]
     L.fslic_b200_set_trace.argtypes = [vp, i32]
     L.fslic_b200_debug_graph_counts.argtypes = [vp, C.POINTER(i32), C.POINTER(i32)]
     L.fslic_b200_trace_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]

@@ -110,7 +110,6 @@ struct fslic_ctx {
     uint8_t* pre_cellmap = nullptr;     // [B][ceil(H/2S) * ceil(W/2S)] active 2S x 2S cells
     int* pre_nactive = nullptr;         // [B] active clusters
     float preempt_l1 = 0.f;             // max(roundf(2 S thres), 1) of the call in progress
-    long long* selprof = nullptr;       // FSLIC_SELPROF=1: 8 words per image written by k_cca_select (diagnostics)
     CcaCounters* h_counters = nullptr;  // pinned, 64 entries: lets the host path learn which images need the replay
     std::vector<cudaEvent_t> pipe_ev;  // [2 * chunks]: input-ready / compute-done events of iterate_host
     // timing
@@ -128,8 +127,7 @@ struct fslic_ctx {
     int kev_used = 0;
     bool kev_on = false;
     bool pending = false;  // an iterate_host_async batch is in flight on this context's streams
-    // small host batches replay one captured CUDA graph per call instead of ~45 launches (FSLIC_GRAPH=0 turns it off)
-    bool graphs_enabled = true;
+    // small host batches replay one captured CUDA graph per call instead of ~45 launches
     cudaGraphExec_t gexec = nullptr;
     struct GraphKey {
         const void *img, *cl, *lab;
@@ -160,7 +158,6 @@ struct fslic_ctx {
     bool lsc_tab_valid = false;
     std::vector<cudaEvent_t> lev;   // start / end events of each after_update launch (collect_timing)
     int lev_used = 0;
-    int assign_impl = 5;       // 5: TMA-staged kernel where it applies (default), 4: always the LDG kernel (FSLIC_ASSIGN=4)
     DispatchRecord disp;       // launch decisions of the last iterate (tests, bench)
     DispatchRecord gdisp;      // ... of the call captured into gexec: a replay makes the same ones
     // debug_mode (fslic_b200_set_trace, trace.cuh): snapshots of the last traced iterate, [B][T] slots, allocated on demand
@@ -270,7 +267,6 @@ extern "C" int fslic_b200_destroy(fslic_ctx* c) {
         if (e) cudaEventDestroy(e);
     if (c->gexec) cudaGraphExecDestroy(c->gexec);
     if (c->h_counters) cudaFreeHost(c->h_counters);
-    if (c->selprof) cudaFree(c->selprof);
     if (c->pre_cellmap) cudaFree(c->pre_cellmap);
     if (c->pre_nactive) cudaFree(c->pre_nactive);
     for (auto& e : c->pipe_ev) cudaEventDestroy(e);
@@ -360,7 +356,6 @@ static int create_impl(int device, int H, int W, int K, int max_batch, bool cca_
         if (v >= 1 && (size_t)v < bc) bc = (size_t)v;
     }
     c->cca_batch = (int)bc;
-    if (const char* e = getenv("FSLIC_GRAPH")) c->graphs_enabled = atoi(e) != 0;
     const int nblk = ceil_div(c->N, CCA_BLOCK);
     CKC(dalloc(&c->par, bc * N));
     CKC(dalloc(&c->aux, bc * N));
@@ -394,12 +389,6 @@ static int create_impl(int device, int H, int W, int K, int max_batch, bool cca_
     CKC(cudaEventCreateWithFlags(&c->tail_done2, cudaEventDisableTiming));
     CKC(cudaEventCreateWithFlags(&c->front_done, cudaEventDisableTiming));
     CKC(cudaMallocHost(reinterpret_cast<void**>(&c->h_counters), 64 * sizeof(CcaCounters)));
-    if (const char* e = getenv("FSLIC_SELPROF")) {
-        if (atoi(e) != 0) {
-            CKC(cudaMalloc(reinterpret_cast<void**>(&c->selprof), (size_t)c->cca_batch * 8 * sizeof(long long)));
-            CKC(cudaMemset(c->selprof, 0, (size_t)c->cca_batch * 8 * sizeof(long long)));
-        }
-    }
 
     // opt in to large dynamic shared memory once
     for (int ts : {128, 192, 256, 384})
@@ -413,7 +402,6 @@ static int create_impl(int device, int H, int W, int K, int max_batch, bool cca_
                 for (int fuse = 0; fuse <= upd; fuse++)
                     CKC(cudaFuncSetAttribute(pick_assign5(ts, upd != 0, tps, fuse != 0), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                              c->max_smem_optin - 1024));
-    if (const char* e = getenv("FSLIC_ASSIGN")) c->assign_impl = atoi(e) == 4 ? 4 : 5;
     CKC(cudaFuncSetAttribute(k_cca_select, cudaFuncAttributeMaxDynamicSharedMemorySize, c->max_smem_optin - 4 * 1024));
     CKC(cudaFuncSetAttribute(k_debug_heap_select, cudaFuncAttributeMaxDynamicSharedMemorySize, c->max_smem_optin - 4 * 1024));
     CKC(cudaFuncSetAttribute(k_prepare, cudaFuncAttributeMaxDynamicSharedMemorySize, 80 * 1024));
@@ -510,7 +498,6 @@ static int run_cca(fslic_ctx* c, const uint16_t* d_in, uint16_t* d_out, int batc
     CcaCounters* const x_counters = c->counters + so;
     unsigned int* const x_ahist = c->ahist + so * CCA_HIST;
     unsigned long long* const x_heap = c->heap + so * (size_t)c->heap_K;
-    long long* const x_selprof = c->selprof ? c->selprof + 8 * so : nullptr;
     CcaCounters* const x_hcnt = c->h_counters + so;
     cudaStream_t const x_side = lane ? c->side_stream2 : c->side_stream;
     cudaEvent_t const x_fork = lane ? c->side_fork2 : c->side_fork, x_join = lane ? c->side_join2 : c->side_join,
@@ -520,8 +507,6 @@ static int run_cca(fslic_ctx* c, const uint16_t* d_in, uint16_t* d_out, int batc
     cp.nblk = ceil_div(N, CCA_BLOCK);
     const size_t heap_bytes = (size_t)(2 * K + 4) * 8;  // live slots + the +infinity padding of the replay loop
     cp.heap_in_smem = heap_bytes + SEL_CHUNK * 8 <= (size_t)(c->max_smem_optin - 8 * 1024);
-    static const int sel_sync = (getenv("FSLIC_SELSYNC") && atoi(getenv("FSLIC_SELSYNC")) == 0) ? 0 : 1;
-    cp.sel_sync = sel_sync;
     if (K + 2 > c->heap_K) return set_err(FSLIC_EINVAL, "K too large for the selection heap");
     c->disp.cca_heap_smem = cp.heap_in_smem ? 1 : 0;
     c->disp.cca_heap_smem_max_k =
@@ -625,7 +610,7 @@ static int run_cca(fslic_ctx* c, const uint16_t* d_in, uint16_t* d_out, int batc
             int rc2 = copy_runs(0);
             if (rc2) return rc2;
         }
-        k_cca_select<<<nb, 1024, SEL_CHUNK * 8 + (cp.heap_in_smem ? heap_bytes : 0), st>>>(cp, x_carea, x_counters, x_heap, x_selprof);
+        k_cca_select<<<nb, 1024, SEL_CHUNK * 8 + (cp.heap_in_smem ? heap_bytes : 0), st>>>(cp, x_carea, x_counters, x_heap);
         tail(split ? 1 : -1, st);
         if (early) {
             CK(cudaEventRecord(x_tail, st));
@@ -939,7 +924,7 @@ static int launch_tma_tiles(fslic_ctx* c, const Slice& sl, AssignParams ap, cons
                             fslic_cluster* fuse_clusters, bool* fused_out, bool* launched) {
     *launched = false;
     const int batch = ap.B, stride = ap.stride;
-    if (!(c->assign_impl == 5 && (c->W % 8) == 0 && g.TS <= 256 && (update ? stride == 3 : stride == 1) &&
+    if (!((c->W % 8) == 0 && g.TS <= 256 && (update ? stride == 3 : stride == 1) &&
           (long)ceil_div(c->W, 32) * ap.tiles_y * batch < (1L << 30) && tensor_map_encoder() != nullptr))
         return FSLIC_OK;
     const size_t tblb = align_up((size_t)g.tbl_elems * 2, 128);
@@ -1542,7 +1527,7 @@ static int iterate_graphed(fslic_ctx* c, const uint8_t* d_images, fslic_cluster*
 extern "C" int fslic_b200_iterate(fslic_ctx* c, const uint8_t* d_images, fslic_cluster* d_clusters, uint16_t* d_labels,
                                   int batch, const fslic_params* p, void* stream) {
     // A traced call launches plainly and leaves the graph and its key alone: the next untraced call replays as before.
-    if (c && p && c->graphs_enabled && !c->trace_on && batch > 0 && batch < 4 && p->collect_timing == 0 && stream != nullptr) {
+    if (c && p && !c->trace_on && batch > 0 && batch < 4 && p->collect_timing == 0 && stream != nullptr) {
         fslic_ctx::GraphKey k;
         graph_key(c, d_clusters, d_labels, batch, p, &k);
         const bool have = c->gexec && memcmp(&k, &c->gkey, sizeof(k)) == 0;
@@ -1625,15 +1610,6 @@ extern "C" int fslic_b200_debug_cca_counters(fslic_ctx* c, int32_t* out8, int im
     USE_DEVICE(c->device);
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(out8, c->counters + image, sizeof(CcaCounters), cudaMemcpyDeviceToHost));
-    return FSLIC_OK;
-}
-
-extern "C" int fslic_b200_debug_select_profile(fslic_ctx* c, long long* out8, int image) {
-    if (!c || !out8 || image < 0 || image >= c->cca_batch) return set_err(FSLIC_EINVAL, "bad argument");
-    if (!c->selprof) return set_err(FSLIC_EINVAL, "the context was created without FSLIC_SELPROF=1");
-    USE_DEVICE(c->device);
-    CK(cudaDeviceSynchronize());
-    CK(cudaMemcpy(out8, c->selprof + 8 * image, 8 * sizeof(long long), cudaMemcpyDeviceToHost));
     return FSLIC_OK;
 }
 
@@ -1792,13 +1768,6 @@ static int iterate_host_enqueue_body(fslic_ctx* c, const uint8_t* h_images, fsli
     if (rc) return rc;
     fslic_params pp = *p;
     if (nchunks > 1) pp.collect_timing = 0;  // per-stage timings are only meaningful for an unchunked run
-    const bool trace = may_sync && getenv("FSLIC_TRACE") != nullptr;
-    std::vector<cudaEvent_t> tev;
-    if (trace) {
-        tev.resize(1 + 4 * nchunks);
-        for (auto& e : tev) cudaEventCreate(&e);
-        cudaEventRecord(tev[0], c->in_stream);
-    }
     for (int k = 0; k < nchunks; k++) {
         const int b0 = k * chunk, nb = (batch - b0 < chunk) ? (batch - b0) : chunk;
         // pipe_ev[3k]: upload of the chunk (of its second half when split), [3k + 2]: of its first half, [3k + 1]: compute
@@ -1821,9 +1790,7 @@ static int iterate_host_enqueue_body(fslic_ctx* c, const uint8_t* h_images, fsli
             for (int h = 0; h < 2; h++) {
                 rc = upload_slice(c, h_images, h_clusters, s0[h], sn[h], up[h]);
                 if (rc) return rc;
-                if (trace && h == 1) cudaEventRecord(tev[1 + 4 * k], c->in_stream);
                 CK(cudaStreamWaitEvent(c->own_stream, up[h], 0));
-                if (trace && h == 0) cudaEventRecord(tev[2 + 4 * k], c->own_stream);
                 // slice s0 - b0 of the context buffers <-> images s0 .. s0+sn of this chunk
                 rc = iterate_front(c, s0[h] - b0, c->d_img + s0[h] * N * 3, c->d_cl + s0[h] * K, sn[h], &pp, coef,
                                    c->own_stream, &launches, false);
@@ -1837,38 +1804,21 @@ static int iterate_host_enqueue_body(fslic_ctx* c, const uint8_t* h_images, fsli
         } else {
             rc = upload_slice(c, h_images, h_clusters, b0, nb, ev[0]);
             if (rc) return rc;
-            if (trace) cudaEventRecord(tev[1 + 4 * k], c->in_stream);
             CK(cudaStreamWaitEvent(c->own_stream, ev[0], 0));
-            if (trace) cudaEventRecord(tev[2 + 4 * k], c->own_stream);
-            if (c->graphs_enabled && nb < 4 && nchunks == 1 && pp.collect_timing == 0)  // nb < 4: one stream, no host sync inside
+            if (nb < 4 && nchunks == 1 && pp.collect_timing == 0)  // nb < 4: one stream, no host sync inside
                 rc = iterate_graphed(c, c->d_img, c->d_cl, c->d_lab, nb, &pp, c->own_stream);
             else
                 rc = iterate_plain(c, c->d_img + b0 * N * 3, c->d_cl + b0 * K, c->d_lab + b0 * N, nb, &pp, c->own_stream);
             if (rc) return rc;
         }
-        if (trace) cudaEventRecord(tev[3 + 4 * k], c->own_stream);
         rc = download_slice(c, h_labels, h_clusters, b0, nb, labels_copied, c->own_stream, ev[1]);
         if (rc) return rc;
-        if (trace) cudaEventRecord(tev[4 + 4 * k], c->out_stream);
     }
     c->pending = true;
     if (!may_sync) return FSLIC_OK;
     CK(cudaStreamSynchronize(c->out_stream));
     CK(cudaStreamSynchronize(c->own_stream));
     c->pending = false;
-    if (trace) {
-        float ms;
-        for (int k = 0; k < nchunks; k++) {
-            float a, b2, c2, d2;
-            cudaEventElapsedTime(&a, tev[0], tev[1 + 4 * k]);
-            cudaEventElapsedTime(&b2, tev[0], tev[2 + 4 * k]);
-            cudaEventElapsedTime(&c2, tev[0], tev[3 + 4 * k]);
-            cudaEventElapsedTime(&d2, tev[0], tev[4 + 4 * k]);
-            fprintf(stderr, "[fslic trace] chunk %d: h2d done %.3f | compute %.3f..%.3f | d2h done %.3f ms\n", k, a, b2, c2, d2);
-        }
-        (void)ms;
-        for (auto e : tev) cudaEventDestroy(e);
-    }
     return FSLIC_OK;
 }
 

@@ -32,7 +32,6 @@ struct CcaParams {
     int thres;         // min_threshold
     int nblk;          // ceil(N / CCA_BLOCK)
     int heap_in_smem;  // k_cca_select keeps its heap in shared memory
-    int sel_sync;      // k_cca_select: warp barriers between the half-steps of the replay loop (FSLIC_SELSYNC, default 1)
     int which;         // post-selection kernels: -1 all images, 0 only images settled by k_cca_threshold, 1 only replayed ones
 };
 
@@ -708,12 +707,10 @@ __device__ __forceinline__ void hs_adjust_heap(const HeapMem<SMEM>& h, int hole,
 // with an earlier sift-down (possible right after a window reload) the hit simply stays where it is and is retried in
 // the next trip -- the root has not changed, and a sift-down ends within `depth` half-steps.
 #define SEL_CHILDREN "ld.volatile.shared.v4.u32 {a0, a1, b0, b1}, [c];\n\t"
-// BAR: "" or a bar.warp.sync behind the store.  The lanes exchange data through shared memory from one half-step to the
-// next; the CUDA memory model asks for a warp barrier in between.  On the hardware a warp's shared-memory instructions
-// execute in issue order and this loop never diverges (everything is predicated, its two branches test vote results),
-// so the barrier-free form computes the same thing ~10 % faster; FSLIC_SELSYNC=0 selects it, the default keeps the
-// barriers (compute-sanitizer racecheck clean).
-#define SEL_HALF_STEP(BAR)                                                                                  \
+// The lanes exchange data through shared memory from one half-step to the next: a lane's store lands in the slot
+// another lane's sift-down loads its children from.  The CUDA memory model orders those accesses only across a warp
+// barrier, hence the bar.warp.sync behind the store.
+#define SEL_HALF_STEP                                                                                       \
     "setp.gt.u32 tl, b1, a1;\n\t"            /* right child unless area[right] > area[left] */             \
     "min.u32 chi, a1, b1;\n\t"                                                                            \
     "selp.b32 clo, a0, b0, tl;\n\t"                                                                       \
@@ -721,7 +718,7 @@ __device__ __forceinline__ void hs_adjust_heap(const HeapMem<SMEM>& h, int hole,
     "min.u32 ohi, chi, vhi;\n\t"                                                                          \
     "selp.b32 olo, clo, vlo, mv;\n\t"                                                                     \
     "@act st.volatile.shared.v2.u32 [hole], {olo, ohi};\n\t" /* ... or the value lands here */             \
-    BAR                                                                                                   \
+    "bar.warp.sync 0xffffffff;\n\t"                                                                      \
     "add.u32 c8, c, 8;\n\t"                                                                               \
     "selp.b32 nh, c, c8, tl;\n\t"                                                                         \
     "selp.b32 hole, nh, rooth, mv;\n\t"      /* idle lanes rest on the root: their loads are one broadcast */ \
@@ -729,12 +726,12 @@ __device__ __forceinline__ void hs_adjust_heap(const HeapMem<SMEM>& h, int hole,
     "sub.u32 c, t0, base;\n\t"               /* slot(h) = h + 1; children at slots 2h+2, 2h+3 */           \
     "mov.pred act, mv;\n\t"
 
-#define SEL_LOOP_ASM(BAR)                                                                                                   \
+#define SEL_LOOP_ASM                                                                                                        \
     "{\n\t"                                                                                                                 \
     ".reg .pred act, mv, tl, p, some, first, nact, take, kill, inq;\n\t"                                                    \
     ".reg .b32 base, c, hole, vlo, vhi, a0, a1, b0, b1, chi, clo, ohi, olo, c8, nh, t0, t1, t2, root, hit, elo, ehi;\n\t"    \
     ".reg .b32 lt, le, wpos, idx, qaddr, rooth, drain;\n\t"                                                                 \
-    "mov.u32 base, %2;\n\t"                                                                                                 \
+    "mov.u32 base, %1;\n\t"                                                                                                 \
     "mov.u32 lt, %%lanemask_lt;\n\t"                                                                                        \
     "mov.u32 le, %%lanemask_le;\n\t"                                                                                        \
     "add.u32 rooth, base, 8;\n\t"     /* root = slot 1, its children = slots 2, 3 */                                        \
@@ -743,22 +740,21 @@ __device__ __forceinline__ void hs_adjust_heap(const HeapMem<SMEM>& h, int hole,
     "mov.u32 vlo, 0;\n\t"                                                                                                   \
     "mov.u32 vhi, 0;\n\t"                                                                                                   \
     "setp.ne.u32 act, 0, 0;\n\t"                                                                                            \
-    "mov.u32 wpos, %5;\n\t"                                                                                                 \
+    "mov.u32 wpos, %4;\n\t"                                                                                                 \
     SEL_CHILDREN                                                                                                            \
     "SEL_LOAD:\n\t"                    /* the window [wpos, wpos + 32) of the queue, one element per lane */                \
-    "add.u32 idx, wpos, %6;\n\t"                                                                                            \
-    "setp.lt.s32 inq, idx, %4;\n\t"                                                                                         \
+    "add.u32 idx, wpos, %5;\n\t"                                                                                            \
+    "setp.lt.s32 inq, idx, %3;\n\t"                                                                                         \
     "mov.u32 elo, 0;\n\t"                                                                                                   \
     "mov.u32 ehi, 0;\n\t"              /* area 0 never beats the root: consumed / missing elements */                       \
     "shl.b32 qaddr, idx, 3;\n\t"                                                                                            \
-    "add.u32 qaddr, qaddr, %3;\n\t"                                                                                         \
+    "add.u32 qaddr, qaddr, %2;\n\t"                                                                                         \
     "@inq ld.shared.v2.u32 {elo, ehi}, [qaddr];\n\t"                                                                        \
     "SEL_TRIP:\n\t"                                                                                                         \
-    "add.u32 %1, %1, 1;\n\t"                                                                                                \
-    SEL_HALF_STEP(BAR)                 /* (its children were loaded at the end of the previous trip) */                     \
+    SEL_HALF_STEP                      /* (its children were loaded at the end of the previous trip) */                     \
     "ld.volatile.shared.u32 root, [base+12];\n\t"  /* final: the newest sift-down has left level 0 */                       \
     SEL_CHILDREN                                                                                                            \
-    SEL_HALF_STEP(BAR)                                                                                                      \
+    SEL_HALF_STEP                                                                                                           \
     "setp.gt.u32 p, ehi, root;\n\t"    /* comp(i, first) of __heap_select */                                                \
     "vote.sync.ballot.b32 hit, p, 0xffffffff;\n\t"                                                                          \
     "vote.sync.any.pred some, p, 0xffffffff;\n\t"                                                                           \
@@ -779,45 +775,36 @@ __device__ __forceinline__ void hs_adjust_heap(const HeapMem<SMEM>& h, int hole,
     "bra.uni SEL_TRIP;\n\t"                                                                                                 \
     "SEL_NEXT:\n\t"                    /* nothing left in the window beats the root, and the root only grows */             \
     "add.u32 wpos, wpos, 32;\n\t"                                                                                           \
-    "setp.lt.s32 inq, wpos, %4;\n\t"                                                                                        \
+    "setp.lt.s32 inq, wpos, %3;\n\t"                                                                                        \
     "@inq bra.uni SEL_LOAD;\n\t"                                                                                            \
-    "mov.u32 drain, %7;\n\t"           /* no sift-down takes more than `depth` half-steps */                                \
+    "mov.u32 drain, %6;\n\t"           /* no sift-down takes more than `depth` half-steps */                                \
     "SEL_DRAIN:\n\t"                                                                                                        \
-    SEL_HALF_STEP(BAR)                                                                                                      \
+    SEL_HALF_STEP                                                                                                           \
     SEL_CHILDREN                                                                                                            \
     "sub.u32 drain, drain, 1;\n\t"                                                                                          \
     "setp.gt.s32 inq, drain, 0;\n\t"                                                                                        \
     "@inq bra.uni SEL_DRAIN;\n\t"                                                                                           \
     "}\n\t"
 
-template <bool WARPSYNC>
-__device__ __forceinline__ int sel_replay_smem(uint32_t heap_saddr, uint32_t queue_saddr, int qn, int consumed, int depth, int lane,
-                                               long long& trips_out) {
-    uint32_t cnt = 0, trips = 0;
+__device__ __forceinline__ int sel_replay_smem(uint32_t heap_saddr, uint32_t queue_saddr, int qn, int consumed, int depth, int lane) {
+    uint32_t cnt = 0;
     if (consumed < qn) {
-        if (WARPSYNC)
-            asm volatile(SEL_LOOP_ASM("bar.warp.sync 0xffffffff;\n\t")
-                         : "+r"(cnt), "+r"(trips)
-                         : "r"(heap_saddr), "r"(queue_saddr), "r"(qn), "r"(consumed), "r"(lane), "r"(depth)
-                         : "memory");
-        else
-            asm volatile(SEL_LOOP_ASM("")
-                         : "+r"(cnt), "+r"(trips)
-                         : "r"(heap_saddr), "r"(queue_saddr), "r"(qn), "r"(consumed), "r"(lane), "r"(depth)
-                         : "memory");
+        asm volatile(SEL_LOOP_ASM
+                     : "+r"(cnt)
+                     : "r"(heap_saddr), "r"(queue_saddr), "r"(qn), "r"(consumed), "r"(lane), "r"(depth)
+                     : "memory");
         __syncwarp();
     }
-    trips_out = trips;
     return (int)__reduce_add_sync(FSLIC_FULL, cnt);
 }
 
 // generic body shared by the pipeline kernel and the debug entry point
-template <bool SMEM, bool WARPSYNC = true>
+template <bool SMEM>
 __device__ __forceinline__ void heap_select_body(const uint32_t* __restrict__ area, int ncomp, int K, int thres,
                                                   const HeapMem<SMEM> heap, uint32_t* __restrict__ mark_out /* |= 1<<31 */,
                                                   uint8_t* __restrict__ kept_bytes /* or nullptr */,
                                                   unsigned long long* s_queue /* shared, SEL_CHUNK entries */,
-                                                  int* dbg_ops = nullptr, long long* prof = nullptr /* 8 words, diagnostics */) {
+                                                  int* dbg_ops = nullptr) {
     __shared__ int s_warp[32];
     __shared__ int s_qn, s_filled;
     __shared__ uint32_t s_min;
@@ -829,7 +816,6 @@ __device__ __forceinline__ void heap_select_body(const uint32_t* __restrict__ ar
     if (SMEM)  // +infinity padding behind the K live slots (see the replay loop)
         for (int u = K + 1 + tid; u < 2 * K + 4; u += nt) heap.put(u, 0u, 0xffffffffu);
     __syncthreads();
-    long long pt_filter = 0, pt_build = 0, pt_replay = 0, pn_iter = 0, pn_queue = 0, pn_chunks = 0, pt0 = clock64(), pt_mark = pt0;
     // thread t owns components base + t*SEL_PER .. +SEL_PER-1 (ascending order inside the thread); the next
     // chunk is prefetched into registers while warp 0 replays the current one
     uint32_t cur[SEL_PER], nxt[SEL_PER];
@@ -883,13 +869,6 @@ __device__ __forceinline__ void heap_select_body(const uint32_t* __restrict__ ar
         }
         __syncthreads();
         const int qn = s_qn;
-        if (prof && tid == 0) {
-            const long long now = clock64();
-            pt_filter += now - pt_mark;
-            pt_mark = now;
-            pn_queue += qn;
-            pn_chunks++;
-        }
         // phase 1: the first K candidates fill the heap array in order
         int consumed = 0;
         if (filling) {
@@ -910,11 +889,6 @@ __device__ __forceinline__ void heap_select_body(const uint32_t* __restrict__ ar
                 __syncthreads();
             }
         }
-        if (prof && tid == 0) {
-            const long long now = clock64();
-            pt_build += now - pt_mark;
-            pt_mark = now;
-        }
         if (f == K && warp == 0) {
             // phase 2: the rest of the queue in order (cca.cpp:226 -> __heap_select loop), as a PIPELINE of
             // sift-downs inside one warp.  Each __pop_heap only ever writes the node it currently stands on
@@ -926,9 +900,7 @@ __device__ __forceinline__ void heap_select_body(const uint32_t* __restrict__ ar
             // levels behind its predecessor), and `depth` half-steps after the last issue everything is done.
             int nops = 0;
             if (SMEM) {
-                long long trips = 0;
-                nops = sel_replay_smem<WARPSYNC>(heap.s, (uint32_t)__cvta_generic_to_shared(s_queue), qn, consumed, 32 - __clz(K), lane, trips);
-                pn_iter += trips;
+                nops = sel_replay_smem(heap.s, (uint32_t)__cvta_generic_to_shared(s_queue), qn, consumed, 32 - __clz(K), lane);
             } else {
             bool act = false;
             int hole = 0;
@@ -983,27 +955,12 @@ __device__ __forceinline__ void heap_select_body(const uint32_t* __restrict__ ar
             if (lane == 0) {
                 s_min = hs_area(heap.get(1));
                 if (dbg_ops) *dbg_ops += nops;
-                if (prof) {
-                    const long long now = clock64();
-                    pt_replay += now - pt_mark;
-                    pt_mark = now;
-                }
             }
         }
         if (tid == 0) s_filled = f;
         __syncthreads();
 #pragma unroll
         for (int u = 0; u < SEL_PER; u++) cur[u] = nxt[u];
-    }
-    if (prof && tid == 0) {
-        prof[0] = clock64() - pt0;
-        prof[1] = pt_filter;
-        prof[2] = pt_build;
-        prof[3] = pt_replay;
-        prof[4] = pn_iter;
-        prof[5] = pn_queue;
-        prof[6] = pn_chunks;
-        prof[7] = ncomp;
     }
     // publish the selected set
     const int filled = s_filled;
@@ -1016,25 +973,23 @@ __device__ __forceinline__ void heap_select_body(const uint32_t* __restrict__ ar
 
 __global__ void __launch_bounds__(1024) k_cca_select(CcaParams cp, uint32_t* __restrict__ carea_all,
                                                      CcaCounters* __restrict__ counters,
-                                                     unsigned long long* __restrict__ heap_global, long long* __restrict__ prof_all) {
+                                                     unsigned long long* __restrict__ heap_global) {
     extern __shared__ __align__(16) unsigned char sel_smem[];  // [queue: SEL_CHUNK x u64][heap: (2K+4) x u64 if it fits]
     unsigned long long* s_queue = reinterpret_cast<unsigned long long*>(sel_smem);
     const int b = blockIdx.x;
     CcaCounters* ct = &counters[b];
     if (!ct->need_sim) return;  // k_cca_threshold settled it (or cca.cpp:225 is not taken)
     uint32_t* area = carea_all + (size_t)b * cp.N;
-    long long* prof = prof_all ? prof_all + 8 * b : nullptr;
     if (cp.heap_in_smem) {
         HeapMem<true> hm;
         hm.g = nullptr;
         hm.s = (uint32_t)__cvta_generic_to_shared(sel_smem + SEL_CHUNK * 8);
-        if (cp.sel_sync) heap_select_body<true, true>(area, ct->ncomp, cp.K, cp.thres, hm, area, nullptr, s_queue, &ct->dbg_ops, prof);
-        else heap_select_body<true, false>(area, ct->ncomp, cp.K, cp.thres, hm, area, nullptr, s_queue, &ct->dbg_ops, prof);
+        heap_select_body<true>(area, ct->ncomp, cp.K, cp.thres, hm, area, nullptr, s_queue, &ct->dbg_ops);
     } else {
         HeapMem<false> hm;
         hm.g = heap_global + (size_t)b * ((cp.K + 3) & ~1);
         hm.s = 0;
-        heap_select_body<false>(area, ct->ncomp, cp.K, cp.thres, hm, area, nullptr, s_queue, &ct->dbg_ops, prof);
+        heap_select_body<false>(area, ct->ncomp, cp.K, cp.thres, hm, area, nullptr, s_queue, &ct->dbg_ops);
     }
     if (threadIdx.x == 0) ct->sel_mode = 1;
 }

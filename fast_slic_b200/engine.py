@@ -245,12 +245,6 @@ class Engine:
         check(self._L.fslic_b200_debug_cca_counters(self._h, out, image))
         return dict(zip(("ncomp", "ncand", "nkept", "sel_mode", "keep_thres", "need_sim", "heap_ops", "kth_area"), list(out)))
 
-    def select_profile(self, image=0):
-        """Clock counts of the std::partial_sort replay (needs FSLIC_SELPROF=1 when the context is created)."""
-        out = (C.c_longlong * 8)()
-        check(self._L.fslic_b200_debug_select_profile(self._h, out, image))
-        return dict(zip(("total", "filter", "build", "replay", "trips", "queued", "chunks", "ncomp"), list(out)))
-
     def assign_impl(self):
         """5: TMA-staged assign kernel, 4: LDG kernel, 0: brute force (last pass of the last iterate)."""
         return int(self._L.fslic_b200_debug_assign_impl(self._h))

@@ -337,11 +337,6 @@ int fslic_b200_assign_kernel_time(fslic_ctx* ctx, float* total_ms, int* launches
  * ncomp, ncand, nkept, sel_mode, keep_thres, need_sim, heap_ops, kth_area. */
 int fslic_b200_debug_cca_counters(fslic_ctx* ctx, int32_t* out8, int image);
 
-/* Diagnostics (contexts created with FSLIC_SELPROF=1 in the environment): 8 int64 words written by the
- * std::partial_sort replay of image `image`: total / filter / heap build / replay clocks, replay loop trips,
- * queued candidates, chunks, components. */
-int fslic_b200_debug_select_profile(fslic_ctx* ctx, long long* out8, int image);
-
 /* Milliseconds spent per stage in the last iterate() with collect_timing != 0. */
 int fslic_b200_stage_ms(fslic_ctx* ctx, float* out_ms, int count);
 
@@ -355,8 +350,8 @@ int fslic_b200_get_S(const fslic_ctx* ctx);
 int fslic_b200_launches_last_iterate(const fslic_ctx* ctx);
 
 /* Diagnostics: which assign kernel the last pass of the last iterate() used -- 5: the TMA-staged kernel
- * (k_assign5; needs W % 8 == 0 and subsample_stride 3), 4: the LDG kernel (k_assign_warp; any shape; forced
- * by the environment variable FSLIC_ASSIGN=4 at context creation), 0: the brute-force kernel / none yet. */
+ * (k_assign5; needs W % 8 == 0 and subsample_stride 3), 4: the LDG kernel (k_assign_warp; any shape, taken where
+ * the TMA-staged kernel does not apply), 0: the brute-force kernel / none yet. */
 int fslic_b200_debug_assign_impl(const fslic_ctx* ctx);
 
 /* Diagnostics: the launch decisions of the last iterate (any iterate entry point, host or device), as the host made

@@ -204,6 +204,19 @@ def test_abi_declares_the_dispatch_read_back():
     assert _lib.DISPATCH_COUNT == 2 * len(_lib.PASS_FIELDS) + 3
 
 
+def test_library_reads_only_the_test_hook_environment_variables():
+    """The library picks every kernel and pipeline from its inputs; the environment only shrinks the connectivity
+    sub-batch and the host chunk, so tests reach those paths with small batches."""
+    csrc = os.path.join(ROOT, "fast_slic_b200", "csrc")
+    calls, names = 0, set()
+    for f in sorted(os.listdir(csrc)):
+        src = open(os.path.join(csrc, f), errors="replace").read()
+        calls += len(re.findall(r"\bgetenv\s*\(", src))
+        names.update(re.findall(r"\bgetenv\s*\(\s*\"(\w+)\"\s*\)", src))
+    assert names == {"FSLIC_CCA_BATCH", "FSLIC_HOST_CHUNK"}
+    assert calls == 2, "getenv with a name that is not a literal, or read in two places"
+
+
 def test_abi_is_sm90a_only():
     out = subprocess.run(["cuobjdump", "--list-elf", os.path.join(ROOT, "fast_slic_b200", "libfslic_b200.so")],
                          capture_output=True, text=True).stdout

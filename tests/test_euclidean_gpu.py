@@ -127,19 +127,18 @@ def test_euclidean_warm_start(euclid):
 LDG_CASES = [c for c in EUCLID_CASES if c[0] in ("pipeline", "dense")]
 
 
-@pytest.mark.parametrize("group,case,seed", LDG_CASES, ids=[case_id(g, c) for g, c, _ in LDG_CASES])
-def test_euclidean_ldg_kernel_forced(euclid, monkeypatch, group, case, seed):
-    """FSLIC_ASSIGN=4: the LDG kernel on images the TMA kernel would take, its list overflow included (dense K)."""
-    from fast_slic_b200 import clear_engine_cache
-    monkeypatch.setenv("FSLIC_ASSIGN", "4")
-    clear_engine_cache()
-    try:
-        name, kind, H, W, K, kw = case
-        sigma, a = split_kwargs(kw)
-        eng = _compare_pipeline(euclid, name, make_image(kind, H, W, seed=seed, sigma=sigma), K, a, 1)
-        assert eng.assign_impl() == 4
-    finally:
-        clear_engine_cache()
+@pytest.mark.parametrize("group,case,seed", LDG_CASES, ids=["%s-W%d" % (case_id(g, c), c[3] - 1) for g, c, _ in LDG_CASES])
+def test_euclidean_ldg_kernel_by_width(euclid, group, case, seed):
+    """The LDG kernel on these shapes one column narrower (W % 8 != 0 rules out the TMA kernel), its list overflow
+    included (dense K)."""
+    name, kind, H, W, K, kw = case
+    W -= 1
+    sigma, a = split_kwargs(kw)
+    img = make_image(kind, H, W, seed=seed, sigma=sigma)
+    eng = _compare_pipeline(euclid, name, img, K, a, 1)
+    assert eng.assign_impl() == 4
+    if group == "dense":
+        assert _max_tile_candidates(euclid.initialize(img, K), eng.S, W) > AS_LIST, "no tile overflows its list"
 
 
 VARIANTS = ("standard", "l2", "noq")

@@ -86,20 +86,16 @@ def test_pipeline_parity_tma_kernel(checker, case):
     assert eng.S > 110 or eng.assign_impl() == 5, "the TMA-staged kernel did not run (impl %d)" % eng.assign_impl()
 
 
-@pytest.mark.parametrize("case", LDG_FORCED_CASES, ids=lambda c: c[0])
-def test_pipeline_parity_ldg_kernel_forced(checker, monkeypatch, case):
-    """FSLIC_ASSIGN=4 keeps the round-1 LDG kernel selectable (it is the path of every W % 8 != 0 image)."""
-    from fast_slic_b200 import clear_engine_cache
-    monkeypatch.setenv("FSLIC_ASSIGN", "4")
-    clear_engine_cache()
-    try:
-        name, kind, H, W, K, kw = case
-        sigma, args = split_kwargs(kw)
-        img = make_image(kind, H, W, seed=29, sigma=sigma)
-        _compare(name, _run_cuda(img, K, args), _run_oracle(checker, img, K, args))
-        assert _engine(H, W, K).assign_impl() in (0, 4)
-    finally:
-        clear_engine_cache()
+@pytest.mark.parametrize("case", LDG_FORCED_CASES, ids=lambda c: "%s-W%d" % (c[0], c[3] - 1))
+def test_pipeline_parity_ldg_kernel_by_width(checker, case):
+    """The round-1 LDG kernel on these shapes one column narrower: W % 8 != 0 rules out the TMA kernel's tensor maps,
+    so the dispatch takes the LDG kernel (the path of every such image) where it would take the TMA one."""
+    name, kind, H, W, K, kw = case
+    W -= 1
+    sigma, args = split_kwargs(kw)
+    img = make_image(kind, H, W, seed=29, sigma=sigma)
+    _compare(name, _run_cuda(img, K, args), _run_oracle(checker, img, K, args))
+    assert _engine(H, W, K).assign_impl() == 4
 
 
 def test_rejects_what_the_reference_cannot_do():
@@ -217,11 +213,10 @@ def test_async_same_context_serialises(checker):
     eng.close()
 
 
-def test_graph_replay_small_host_batches(checker, monkeypatch):
-    """Host calls with fewer than 4 images replay one captured CUDA graph (default; FSLIC_GRAPH=0 disables).  Same
-    results as the plain launches for changing images (replay), changing parameters (re-capture) and the async entry point."""
+def test_graph_replay_small_host_batches(checker):
+    """Host calls with fewer than 4 images replay one captured CUDA graph.  Same results as the plain launches for
+    changing images (replay), changing parameters (re-capture) and the async entry point."""
     from fast_slic_b200 import Engine
-    monkeypatch.setenv("FSLIC_GRAPH", "1")
     H, W, K = 120, 160, 40
     eng = Engine(H, W, K, 2)
     for msf in (0.0, 0.3):

@@ -91,10 +91,9 @@ def main(lib_path, out_path):
             out[name] = record(eng, lab, cl, **extra)
             eng.close()
 
-    # the u16 path: TMA (W % 8 == 0, stride 3), LDG (FSLIC_ASSIGN=4 or W % 8 != 0), generic (S > 160: no patch in smem)
+    # the u16 path: TMA (W % 8 == 0, stride 3), LDG (W % 8 != 0), generic (S > 160: no patch in smem)
     for B in (1, 2, 8, 32):
         device_run("tma_b%d" % B, 240, 320, 300, B)
-        device_run("ldg_b%d" % B, 240, 320, 300, B, env={"FSLIC_ASSIGN": "4"})
         device_run("generic_b%d" % B, 400, 400, 4, B)
     device_run("w_mod8_b1", 241, 323, 300, 1)
     device_run("w_mod8_b8", 241, 323, 300, 8)
@@ -155,7 +154,6 @@ def main(lib_path, out_path):
 
     for B in (1, 3, 8, 16, 32, 40):
         host_run("host_b%d" % B, B, calls=2)
-    host_run("host_nograph_b1", 1, env={"FSLIC_GRAPH": "0"})
     host_run("host_timing_b2", 2, collect_timing=1)
     host_run("host_chunk4_b8", 8, env={"FSLIC_HOST_CHUNK": "4"})
     host_run("host_chunk8_b24", 24, env={"FSLIC_HOST_CHUNK": "8"})
