@@ -38,12 +38,13 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_crfgroup_inference", "fslic_b200_crfdev_group_push_label_frames", "fslic_b200_crfdev_group_set_proba",
     "fslic_b200_crfdev_group_reset_inferred", "fslic_b200_crfdev_group_get_inferred", "fslic_b200_crfgroup_pop_frame",
     "fslic_b200_pool_batch_scratch_bytes", "fslic_b200_pool_batch", "fslic_b200_pool_unpool_batch",
-    "fslic_b200_pool_paint_argmax_batch",
+    "fslic_b200_pool_paint_argmax_batch", "fslic_b200_pool_paint_batch",
     "fslic_b200_rag_batch_scratch_bytes", "fslic_b200_rag_batch_count", "fslic_b200_rag_fill_scratch_bytes",
     "fslic_b200_rag_batch_fill",
     "fslic_b200_gt_histogram_batch", "fslic_b200_gt_scores_scratch_bytes", "fslic_b200_gt_scores_batch",
     "fslic_b200_gt_boundaries_batch",
     "fslic_b200_props_batch",
+    "fslic_b200_merge_scratch_bytes", "fslic_b200_merge_batch",
 )
 
 STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity", "iterate")
@@ -127,6 +128,7 @@ def lib():
     L.fslic_b200_pool_batch.argtypes = [i32, i32, i32, i32, i32, i32, vp, vp, i32, vp, vp, vp, C.c_size_t, vp]
     L.fslic_b200_pool_unpool_batch.argtypes = [i32, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp]
     L.fslic_b200_pool_paint_argmax_batch.argtypes = [i32, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp]
+    L.fslic_b200_pool_paint_batch.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp]
     i64 = C.c_longlong
     L.fslic_b200_rag_batch_scratch_bytes.argtypes = [i32, i32, i32, i32, i32, i32]
     L.fslic_b200_rag_batch_scratch_bytes.restype = C.c_size_t
@@ -142,6 +144,10 @@ def lib():
                                              vp]
     L.fslic_b200_gt_boundaries_batch.argtypes = [i32, i32, i32, i32, vp, vp, vp]
     L.fslic_b200_props_batch.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.fslic_b200_merge_scratch_bytes.argtypes = [i32, i32]
+    L.fslic_b200_merge_scratch_bytes.restype = C.c_size_t
+    L.fslic_b200_merge_batch.argtypes = [i32, i32, i32, i32, i32, vp, i64, vp, vp, vp, i32, C.c_double, i32, vp, vp, vp,
+                                         vp, C.c_size_t, vp]
     L.fslic_b200_assign_kernel_time.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]
     L.fslic_b200_debug_cca_counters.argtypes = [vp, C.POINTER(C.c_int32), i32]
     L.fslic_b200_set_trace.argtypes = [vp, i32]

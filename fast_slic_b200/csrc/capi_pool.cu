@@ -1,6 +1,6 @@
-// fast_slic_b200/csrc/capi_pool.cu -- the extern "C" entry points of superpixel pooling (pool.cuh): pool, unpool and
-// paint_argmax over a batch of label maps.  Stateless (device pointers, caller-provided scratch), asynchronous on the
-// caller's stream, never synchronise.
+// fast_slic_b200/csrc/capi_pool.cu -- the extern "C" entry points of superpixel pooling (pool.cuh): pool, unpool,
+// paint_argmax and paint over a batch of label maps.  Stateless (device pointers, caller-provided scratch), asynchronous
+// on the caller's stream, never synchronise.
 #include <limits.h>
 
 #include <cub/device/device_radix_sort.cuh>
@@ -92,6 +92,18 @@ extern "C" int fslic_b200_pool_paint_argmax_batch(int device, int batch, int H, 
     const long nk = (long)batch * K;
     k_pool_node_argmax<<<(int)grid_for(nk, device), 256, 0, st>>>(d_q, nk, C, K, d_node_class);
     k_pool_paint<<<(int)grid_for(n, device), 256, 0, st>>>(d_labels, d_node_class, (long)H * W, n, K, d_out);
+    CK(cudaGetLastError());
+    return FSLIC_OK;
+}
+
+extern "C" int fslic_b200_pool_paint_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels,
+                                          const int32_t* d_table, int16_t* d_out, void* stream) {
+    if (!pool_shape_ok(batch, H, W, K)) return set_err(FSLIC_EINVAL, "bad batch, H, W or K");
+    const long n = (long)batch * H * W;
+    if (n == 0) return FSLIC_OK;
+    if (!d_labels || !d_table || !d_out) return set_err(FSLIC_EINVAL, "NULL argument");
+    USE_DEVICE(device);
+    k_pool_paint<<<(int)grid_for(n, device), 256, 0, (cudaStream_t)stream>>>(d_labels, d_table, (long)H * W, n, K, d_out);
     CK(cudaGetLastError());
     return FSLIC_OK;
 }

@@ -239,6 +239,9 @@ int fslic_b200_pool_unpool_batch(int device, int batch, int H, int W, int C, int
  * counts as the maximum), -1 where the label is outside [0, K); C <= 32767.  d_node_class: int32[B,K] scratch. */
 int fslic_b200_pool_paint_argmax_batch(int device, int batch, int H, int W, int C, int K, const uint16_t* d_labels,
                                        const float* d_q, int32_t* d_node_class, int16_t* d_out, void* stream);
+/* d_table int32[B,K] -> d_out int16[B,H,W]: (int16)d_table[b,label] at each pixel, -1 where the label is outside [0, K). */
+int fslic_b200_pool_paint_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels,
+                                const int32_t* d_table, int16_t* d_out, void* stream);
 
 /* Region adjacency graphs (rag.cuh; no counterpart in the reference) of `batch` label maps d_labels u16[B,H,W]: node
  * b*K + k is label k of image b; an edge joins two labels of one image for every unordered pair of adjacent pixels
@@ -314,6 +317,34 @@ int fslic_b200_gt_boundaries_batch(int device, int batch, int H, int W, const ui
 int fslic_b200_props_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels, int32_t* d_area,
                            int32_t* d_bbox, long long* d_moments, int32_t* d_perimeter, int32_t* d_border,
                            double* d_centroid, double* d_covariance, void* stream);
+
+/* Superpixels merged into regions (merge.cuh; no counterpart in the reference): single-linkage cuts of a region
+ * adjacency graph over `batch` label maps d_labels u16[B,H,W].  Node n = b*K + k is label k of image b, present when a
+ * pixel of image b carries k.  1 <= K <= 65534, B * K <= 2^30.
+ * Edges: d_src / d_dst int64[E] and d_weight f32[E].  Only entries with src < dst are read, and the weight of the
+ * undirected edge {src, dst} is the weight of that entry.  An entry is ignored when an endpoint is outside [0, B*K),
+ * the endpoints lie in different images, an endpoint is not present or the weight is NaN.
+ * Order: edges by (weight, lower local id, higher local id), -0.0 equal to +0.0; single linkage is Kruskal over it.
+ *   FSLIC_MERGE_THRESHOLD: two nodes share a region exactly when a path of edges with (double)weight < threshold joins
+ *     them (threshold not NaN).
+ *   FSLIC_MERGE_NUM_REGIONS: Kruskal stops after P_b - num_regions merges or when it runs out of edges (P_b: the present
+ *     nodes of image b; num_regions >= 1), leaving max(num_regions, c_b) regions where c_b is the number of connected
+ *     components among present nodes over non-NaN edges.
+ * Outputs: d_region int32[B,K], the region of node b*K + k, regions of an image numbered 0, 1, ... in ascending order of
+ * their smallest member, -1 for a node that is not present; d_num_regions int32[B]; d_out int16[B,H,W], the region of
+ * each pixel's label (fslic_b200_pool_paint_batch of d_region), -1 where the label is outside [0, K).
+ * Integer arithmetic once each weight is a key, so the result of image b depends on its labels and edges only.
+ * Asynchronous on `stream`, never synchronises and reads nothing back (a CUDA graph can capture it); batch == 0 does
+ * nothing.  DESIGN.md section 4.16 describes the kernels.
+ * Scratch bytes: 40 per node, 16 per image, the Boruvka round flags and the larger temporary storage of the segmented
+ * radix sort and the scan, each piece aligned to 256; (size_t)-1 for a bad K or B * K > 2^30. */
+#define FSLIC_MERGE_THRESHOLD 0
+#define FSLIC_MERGE_NUM_REGIONS 1
+size_t fslic_b200_merge_scratch_bytes(int batch, int K);
+int fslic_b200_merge_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels, long long edges,
+                           const long long* d_src, const long long* d_dst, const float* d_weight, int mode,
+                           double threshold, int num_regions, int32_t* d_region, int32_t* d_num_regions,
+                           int16_t* d_out, void* d_scratch, size_t scratch_bytes, void* stream);
 
 /* Stage probes for the parity tests (the reference's protected quad_image / assignment,
  * context.h:48-50): copies of the last iterate()'s Lab quad image [B,H,W,4] u8 and pre-CCA
