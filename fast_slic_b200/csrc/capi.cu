@@ -127,6 +127,7 @@ struct fslic_ctx {
     int kev_used = 0;
     bool kev_on = false;
     bool pending = false;  // an iterate_host_async batch is in flight on this context's streams
+    cudaEvent_t last_work = nullptr;  // end of the last call's device work on this context (CtxOrder)
     // small host batches replay one captured CUDA graph per call instead of ~45 launches
     cudaGraphExec_t gexec = nullptr;
     struct GraphKey {
@@ -243,6 +244,7 @@ static cudaError_t dalloc(T** p, size_t count) {
 extern "C" int fslic_b200_destroy(fslic_ctx* c) {
     if (!c) return FSLIC_OK;
     DeviceGuard dev_guard__(c->device);
+    if (c->last_work) cudaEventSynchronize(c->last_work);  // the last call may still be running on a caller's stream
     void* ptrs[] = {c->d_gamma, c->d_labtbl, c->quad,   c->labels,  c->cinfo,  c->acc,    c->cell_start,
                     c->cinfo_tmp, c->cell_cnt, c->prep_tickets, c->sptable, c->par,  c->aux,    c->predbuf, c->carea,
                     c->cnew,    c->chunkinfo, c->rootbuf, c->blkcnt, c->blkoff,  c->kblkoff, c->counters, c->ahist, c->heap, c->d_img,
@@ -263,7 +265,7 @@ extern "C" int fslic_b200_destroy(fslic_ctx* c) {
     if (c->tail_done) cudaEventDestroy(c->tail_done);
     if (c->own_stream2) cudaStreamDestroy(c->own_stream2);
     if (c->side_stream2) cudaStreamDestroy(c->side_stream2);
-    for (cudaEvent_t e : {c->side_fork2, c->side_join2, c->tail_done2, c->front_done})
+    for (cudaEvent_t e : {c->side_fork2, c->side_join2, c->tail_done2, c->front_done, c->last_work})
         if (e) cudaEventDestroy(e);
     if (c->gexec) cudaGraphExecDestroy(c->gexec);
     if (c->h_counters) cudaFreeHost(c->h_counters);
@@ -388,6 +390,7 @@ static int create_impl(int device, int H, int W, int K, int max_batch, bool cca_
     CKC(cudaEventCreateWithFlags(&c->side_join2, cudaEventDisableTiming));
     CKC(cudaEventCreateWithFlags(&c->tail_done2, cudaEventDisableTiming));
     CKC(cudaEventCreateWithFlags(&c->front_done, cudaEventDisableTiming));
+    CKC(cudaEventCreateWithFlags(&c->last_work, cudaEventDisableTiming));
     CKC(cudaMallocHost(reinterpret_cast<void**>(&c->h_counters), 64 * sizeof(CcaCounters)));
 
     // opt in to large dynamic shared memory once
@@ -419,6 +422,39 @@ extern "C" int fslic_b200_create(int device, int H, int W, int K, int max_batch,
 extern "C" int fslic_b200_create_cca(int device, int H, int W, int max_batch, fslic_ctx** out) {
     return create_impl(device, H, W, 1, max_batch, true, out);
 }
+
+// ---- order between calls on one context ----------------------------------------------------------------------
+// The scratch above belongs to the context, not to a call, and calls may come on any stream: the device entry points
+// enqueue on the caller's, the host ones on the context's own non-blocking streams.  So every entry point that touches
+// the scratch first makes each stream it computes on wait for `last_work`, and records its own end there: consecutive
+// calls on one context run one after the other on the device, whatever streams they use.  A stream that is being
+// captured into a CUDA graph neither waits nor records (the capture cannot depend on outside work); fslic_b200_iterate
+// waits before iterate_graphed begins its capture and records after the graph's launch.
+static bool stream_capturing(cudaStream_t st) {
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    return cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap != cudaStreamCaptureStatusNone;
+}
+
+// Waits for the context's last work on `st` when constructed and, when the call returns, records the call's end on
+// `join` (the stream where all of its work comes together; `st` for the device entry points), on every return path:
+// work enqueued before an error is ordered too.
+struct CtxOrder {
+    fslic_ctx* c;
+    cudaStream_t join;
+    bool on;
+    cudaError_t err = cudaSuccess;
+    CtxOrder(fslic_ctx* c_, cudaStream_t st, cudaStream_t join_) : c(c_), join(join_), on(!stream_capturing(st)) {
+        if (on) err = cudaStreamWaitEvent(st, c->last_work, 0);
+    }
+    ~CtxOrder() {
+        if (on && err == cudaSuccess && cudaEventRecord(c->last_work, join) != cudaSuccess) cudaGetLastError();
+    }
+};
+#define ORDER_CALL_JOIN(c, st, join)                                                                  \
+    CtxOrder ctx_order__(c, st, join);                                                                \
+    if (ctx_order__.err != cudaSuccess)                                                               \
+        return set_err(FSLIC_ECUDA, std::string("cudaStreamWaitEvent: ") + cudaGetErrorString(ctx_order__.err))
+#define ORDER_CALL(c, st) ORDER_CALL_JOIN(c, st, st)
 
 static int check_batch(fslic_ctx* c, int batch, bool needs_assign_state = true) {
     if (!c) return set_err(FSLIC_EINVAL, "ctx is NULL");
@@ -636,6 +672,7 @@ extern "C" int fslic_b200_enforce_connectivity(fslic_ctx* c, uint16_t* d_labels,
     if (K <= 0) return FSLIC_OK;  // context.cpp:17
     if (K > 65535) return set_err(FSLIC_EINVAL, "K must fit the u16 label type");
     USE_DEVICE(c->device);
+    ORDER_CALL(c, (cudaStream_t)stream);
     c->disp = DispatchRecord();
     return run_cca(c, d_labels, d_labels, batch, K, min_threshold, (cudaStream_t)stream, nullptr);
 }
@@ -645,6 +682,7 @@ extern "C" int fslic_b200_debug_heap_select(fslic_ctx* c, const int32_t* d_area,
     if (!c) return set_err(FSLIC_EINVAL, "ctx is NULL");
     if (middle + 2 > c->heap_K || middle < 1 || n < 1) return set_err(FSLIC_EINVAL, "bad n/middle");
     USE_DEVICE(c->device);
+    ORDER_CALL(c, (cudaStream_t)stream);
     CK(cudaMemsetAsync(d_kept, 0, n, (cudaStream_t)stream));
     const size_t hb = (size_t)(2 * middle + 4) * 8;
     const int use_smem = hb + SEL_CHUNK * 8 <= (size_t)(c->max_smem_optin - 8 * 1024);
@@ -804,7 +842,7 @@ static int build_patches(fslic_ctx* c, int stride, bool need_sub, float coef, cu
                       c->spt_coef_bits == coef_bits && c->spt_manhattan == c->manhattan && (c->spt_has_sub || !need_sub);
     if (warm) return FSLIC_OK;
     c->spt_valid = true;
-    c->spt_stream = st;  // a call on another stream is not ordered after this build: it rebuilds
+    c->spt_stream = st;  // a call on another stream rebuilds (ordered after this build by CtxOrder all the same)
     c->spt_stride = stride;
     c->spt_coef_bits = coef_bits;
     c->spt_manhattan = c->manhattan;
@@ -1526,6 +1564,9 @@ static int iterate_graphed(fslic_ctx* c, const uint8_t* d_images, fslic_cluster*
 // from then on.  Needs a capturable stream (not the legacy default stream) and no timing; anything else launches plainly.
 extern "C" int fslic_b200_iterate(fslic_ctx* c, const uint8_t* d_images, fslic_cluster* d_clusters, uint16_t* d_labels,
                                   int batch, const fslic_params* p, void* stream) {
+    if (!c) return set_err(FSLIC_EINVAL, "ctx is NULL");
+    // (the wait is enqueued before iterate_graphed begins a capture: the graph's launch waits, the graph itself does not)
+    ORDER_CALL(c, (cudaStream_t)stream);
     // A traced call launches plainly and leaves the graph and its key alone: the next untraced call replays as before.
     if (c && p && !c->trace_on && batch > 0 && batch < 4 && p->collect_timing == 0 && stream != nullptr) {
         fslic_ctx::GraphKey k;
@@ -1543,6 +1584,8 @@ extern "C" int fslic_b200_iterate(fslic_ctx* c, const uint8_t* d_images, fslic_c
 extern "C" int fslic_b200_iterate_real(fslic_ctx* c, int variant, const uint8_t* d_images, fslic_cluster* d_clusters,
                                        uint16_t* d_labels, int batch, const fslic_params* p, void* stream) {
     if (variant < 0 || variant > 2) return set_err(FSLIC_EINVAL, "variant must be 0 (standard), 1 (l2) or 2 (noq)");
+    if (!c) return set_err(FSLIC_EINVAL, "ctx is NULL");
+    ORDER_CALL(c, (cudaStream_t)stream);
     return iterate_plain(c, d_images, d_clusters, d_labels, batch, p, stream, false, (AssignPath)variant);
 }
 
@@ -1554,6 +1597,7 @@ extern "C" int fslic_b200_iterate_lsc(fslic_ctx* c, const uint8_t* d_images, fsl
     USE_DEVICE(c->device);
     rc = ensure_lsc(c);
     if (rc) return rc;
+    ORDER_CALL(c, (cudaStream_t)stream);
     return iterate_plain(c, d_images, d_clusters, d_labels, batch, p, stream, false, PATH_LSC);
 }
 
@@ -1564,6 +1608,7 @@ extern "C" int fslic_b200_debug_lsc_stages(fslic_ctx* c, float* d_means_out, flo
     if (!c->lsc_feat) return set_err(FSLIC_EINVAL, "no LSC iterate has run on this context");
     USE_DEVICE(c->device);
     cudaStream_t st = (cudaStream_t)stream;
+    ORDER_CALL(c, st);
     if (d_means_out)
         CK(cudaMemcpyAsync(d_means_out, c->lsc_means, sizeof(float) * LSC_NF * batch, cudaMemcpyDeviceToDevice, st));
     if (d_weights_out)
@@ -1595,6 +1640,7 @@ extern "C" int fslic_b200_iterate_preemptive(fslic_ctx* c, const uint8_t* d_imag
         c->pre_nactive = na;
     }
     c->preempt_l1 = fmaxf(roundf((float)(2 * c->S) * preemptive_thres), 1.0f);  // preemptive.h:126
+    ORDER_CALL(c, (cudaStream_t)stream);
     return iterate_plain(c, d_images, d_clusters, d_labels, batch, p, stream, false, PATH_PREEMPTIVE);
 }
 
@@ -1625,6 +1671,7 @@ extern "C" int fslic_b200_debug_stages(fslic_ctx* c, uint8_t* d_quad_out, uint16
     if (rc) return rc;
     USE_DEVICE(c->device);
     cudaStream_t st = (cudaStream_t)stream;
+    ORDER_CALL(c, st);
     if (d_quad_out) CK(cudaMemcpyAsync(d_quad_out, c->quad, (size_t)batch * c->N * 4, cudaMemcpyDeviceToDevice, st));
     if (d_precca_out) CK(cudaMemcpyAsync(d_precca_out, c->labels, (size_t)batch * c->N * 2, cudaMemcpyDeviceToDevice, st));
     return FSLIC_OK;
@@ -1662,6 +1709,7 @@ extern "C" int fslic_b200_initialize_clusters_host(fslic_ctx* c, const uint8_t* 
     rc = ensure_staging(c);
     if (rc) return rc;
     cudaStream_t st = c->own_stream;
+    ORDER_CALL(c, st);
     const size_t ib = (size_t)batch * c->N * 3, cb = (size_t)batch * c->K * sizeof(fslic_cluster);
     CK(cudaMemcpyAsync(c->d_img, h_images, ib, cudaMemcpyHostToDevice, st));
     rc = fslic_b200_initialize_clusters(c, c->d_img, c->d_cl, batch, st);
@@ -1707,6 +1755,7 @@ static int iterate_host_lanes(fslic_ctx* c, const uint8_t* h_images, fslic_clust
     cudaStream_t const cs[2] = {c->own_stream, c->own_stream2};
     cudaEvent_t const up[2] = {c->pipe_ev[2], c->pipe_ev[0]};
     int launches = 0, rc;
+    CK(cudaStreamWaitEvent(c->own_stream2, c->last_work, 0));
     for (int h = 0; h < 2; h++) {
         rc = upload_slice(c, h_images, h_clusters, s0[h], sn[h], up[h]);
         if (rc) return rc;
@@ -1751,6 +1800,10 @@ static int iterate_host_enqueue_body(fslic_ctx* c, const uint8_t* h_images, fsli
         CK(cudaStreamSynchronize(c->own_stream));
         c->pending = false;
     }
+    // The compute streams start behind the context's last work (own_stream2 in iterate_host_lanes); the call's work
+    // joins on out_stream, behind the label and cluster downloads.  in_stream only fills the staging buffers, which no
+    // other call touches while this one runs: host calls wait for a pending one above, device calls never use them.
+    ORDER_CALL_JOIN(c, c->own_stream, c->out_stream);
     c->disp = DispatchRecord();
     // Software pipeline over chunks of the batch: H2D(chunk i+1) | compute(chunk i) | D2H(chunk i-1) on three
     // streams, so for batches the PCIe copies hide behind the kernels (and vice versa).  With pinned host

@@ -29,8 +29,10 @@ def require_cuda():
 
 
 class Engine:
-    """A context is NOT safe for concurrent calls (shared staging buffers, streams, graph key; INTEGRATION.md).
-    `lock` serialises them: every blocking entry point below holds it for the whole call, and callers that pair
+    """Consecutive calls on one context are ordered on the device whatever streams they use: a call enqueued on one
+    stream runs after the context's previous call on any other stream or on the host path (INTEGRATION.md section 4).
+    The host side is NOT safe for concurrent calls (shared staging buffers, streams, graph key): `lock` serialises
+    calls from several threads.  Every blocking entry point below holds it for the whole call, and callers that pair
     `iterate_host_async` with `wait` from several threads must hold it across the pair themselves."""
 
     def __init__(self, H, W, K=None, max_batch=1, device=0, cca_only=False):
