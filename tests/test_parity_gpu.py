@@ -102,10 +102,14 @@ def test_rejects_what_the_reference_cannot_do():
     """K > H*W makes S = 0: the reference divides by zero there (preemptive.h:37-38); compactness beyond the u16
     distance range is undefined behaviour in the reference (context.cpp:30).  Both are refused, not guessed."""
     from fast_slic_b200 import Slic
+    from fast_slic_b200._lib import FslicError
     with pytest.raises(ValueError):
         Slic(num_components=50).iterate(np.zeros((6, 6, 3), np.uint8))
-    with pytest.raises(Exception):
-        Slic(num_components=30, compactness=1e6).iterate(np.zeros((64, 64, 3), np.uint8))
+    # (the exact bound, and that a refused call writes nothing: tests/test_default_sweep_gpu.py)
+    for lab in (True, False):
+        s = Slic(num_components=30, compactness=1e6, convert_to_lab=lab)
+        with pytest.raises(FslicError, match="compactness too large"):
+            s.iterate(np.zeros((64, 64, 3), np.uint8))
 
 
 @pytest.mark.parametrize("case", BIG_CASES, ids=[c[0] for c in BIG_CASES])
