@@ -34,6 +34,7 @@
 #include <cuda.h>  // CUtensorMap (types only; the encoder is fetched through cudaGetDriverEntryPoint, no libcuda link)
 
 #include "assign.cuh"
+#include "prepare.cuh"
 
 #define A5_MAXWARPS 32
 #define A5_WBLK 5504     // bytes of shared memory per warp (multiple of 128: TMA destinations need 128-byte alignment)
@@ -519,19 +520,9 @@ __global__ void __launch_bounds__(32 * A5_MAXWARPS, 1)
         // Small batches: the bookkeeping between two passes (k_prepare3's work) runs right here, in the last CTA to
         // finish, instead of in a kernel of its own.  cinfo_next / cell_start_next alias cinfo / cell_start: they are
         // written only after every CTA of the grid has taken its ticket, i.e. has read them for the last time.
-        __shared__ int s_last;
-        __threadfence();  // this thread's RED.64 are performed before its CTA's ticket is
-        __syncthreads();
-        if (threadIdx.x == 0) s_last = (atomicAdd(ticket, 1u) == gridDim.x - 1u) ? 1 : 0;
-        __syncthreads();
-        if (s_last) {
-            if (threadIdx.x == 0) *ticket = 0u;  // zero between launches
-            __threadfence();
-            PrepParams pp;
-            pp.H = ap.H; pp.W = ap.W; pp.K = ap.K; pp.S = ap.S; pp.T = 2 * ap.S + 32;
-            pp.G = ap.G; pp.cellW = ap.cellW; pp.cellH = ap.cellH; pp.ncell = ap.ncell;
-            pp.first = 0; pp.finalize = 1; pp.last = 0; pp.noq = 0;
-            pp.preempt = 0; pp.l1_thres = 0.f; pp.nactive = nullptr;
+        if (last_block_to_arrive(ticket, gridDim.x)) {  // its first fence performs this thread's RED.64 before the ticket
+            PrepParams pp = prep_params(ap.H, ap.W, ap.K, ap.S, ap.G, ap.cellW, ap.cellH, ap.ncell);
+            pp.finalize = 1;
             for (int bi = 0; bi < ap.B; bi++)
                 prepare_in_tail(pp, clusters + (size_t)bi * ap.K, acc + (size_t)bi * ap.K * 4, cinfo_next + (size_t)bi * ap.K,
                                 cell_start_next + (size_t)bi * (ap.ncell + 1), smem_raw, (int)threadIdx.x, (int)blockDim.x);

@@ -1098,9 +1098,7 @@ static int run_assign_pass(fslic_ctx* c, const Slice& sl, int batch, int stride,
 
 static int run_prepare(fslic_ctx* c, const Slice& sl, fslic_cluster* d_clusters, int batch, int first, int finalize,
                        cudaStream_t st, int* launches, int noq = 0, int preempt = 0, int last = 0) {
-    PrepParams pp;
-    pp.H = c->H; pp.W = c->W; pp.K = c->K; pp.S = c->S; pp.T = 2 * c->S + 32;
-    pp.G = c->G; pp.cellW = c->cellW; pp.cellH = c->cellH; pp.ncell = c->ncell;
+    PrepParams pp = prep_params(c->H, c->W, c->K, c->S, c->G, c->cellW, c->cellH, c->ncell);
     pp.first = first; pp.finalize = finalize; pp.last = last; pp.noq = noq;
     pp.preempt = preempt; pp.l1_thres = c->preempt_l1; pp.nactive = preempt ? sl.pre_nactive : nullptr;
     const size_t smem = (size_t)(c->ncell + 2) * sizeof(int);

@@ -8,10 +8,12 @@
 // them), pixels of inactive cells do not count in the next update, clusters that are not updatable keep their centre.
 //
 // It is an option that is off in every BASELINE configuration, so this is a correctness-first path (one thread per
-// pixel over the cell grid, like k_assign_generic); the bookkeeping rides on k_prepare (PrepParams.preempt) plus
-// k_preempt_mark below.  Results are bit-identical to the compiled reference (tests/test_parity_gpu.py).
+// pixel over the cell grid, like k_assign_generic); the bookkeeping rides on k_prepare (prepare.cuh: PrepParams.preempt,
+// the PREEMPT rules of finalize_cluster and clamp_cluster) plus k_preempt_mark below.  Results are bit-identical to the
+// compiled reference (tests/test_parity_gpu.py).
 #pragma once
 #include "assign.cuh"
+#include "prepare.cuh"
 
 // per image: is_active of every cluster, the active-cell map and the number of active clusters.  One CTA per image.
 // cinfo / cell_start: the FULL cell grid k_prepare just built (all clusters, new centres).
