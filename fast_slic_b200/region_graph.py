@@ -6,8 +6,14 @@ CSR / COO layout graph libraries take.  With pooling.pool it gives a superpixel 
     g = region_adjacency(labels, K)                      # the B*K nodes' graph, one block per image
     A = torch.sparse_csr_tensor(g.indptr, g.edge_index[1], g.boundary.float(), (B * K, B * K))
 
+boundary_stats gives each edge the mean, min and max of pixel maps along its shared boundary (PyG's edge_attr), such
+as the strength of an edge map between two superpixels, which merging.merge_regions takes as its weights::
+
+    s = boundary_stats(labels, K, g, edge_map[:, None])  # [E,1] mean / min / max, [E] pair counts
+    m = merge_regions(labels, K, g, s.mean[:, 0], threshold=t)
+
 No counterpart in the reference: its get_connectivity keeps at most 12 neighbours per superpixel, in scan order, and
-is kept for parity with it.  DESIGN.md section 4.13 describes the kernels.
+is kept for parity with it.  DESIGN.md sections 4.13 and 4.17 describe the kernels.
 """
 import collections
 import operator
@@ -20,12 +26,18 @@ from .pooling import _check_K, _tensor  # the K range of pooling.MAX_K
 # Device memory the pair tables of one count launch take at most (8 bytes per slot, a power of two >= max(4096, 32 K)
 # slots per image): a batch that needs more runs in chunks of images, with identical results.
 RAG_SCRATCH_CAP = 1 << 30
+# Device memory the boundary pair selection of one launch takes at most (4 bytes per pixel pair, 2 or 4 per pixel),
+# sized before the pair count is known: a batch that needs more runs in chunks of images, with identical results.  A
+# chunk whose boundary pairs need more than this for their sort is split again (only maps that are not superpixel maps,
+# such as noise, have that many).
+BOUNDARY_SCRATCH_CAP = 1 << 30
 # Larger images could have a boundary count above int32
 MAX_PIXELS = 1 << 29
 _INT_MAX = 2 ** 31 - 1
 _NO_SIZE = 2 ** 64 - 1
 
 RegionGraph = collections.namedtuple("RegionGraph", ["indptr", "edge_index", "boundary"])
+BoundaryStats = collections.namedtuple("BoundaryStats", ["mean", "min", "max", "count"])
 
 
 def rag_chunk(B, H, W, K, connectivity):
@@ -57,6 +69,16 @@ def _split(b0, flags):
     return runs
 
 
+def _check_connectivity(connectivity):
+    try:
+        connectivity = operator.index(connectivity)
+    except TypeError:
+        raise ValueError("connectivity must be 4 or 8, got %r" % (connectivity,)) from None
+    if connectivity not in (4, 8):
+        raise ValueError("connectivity must be 4 or 8, got %r" % (connectivity,))
+    return connectivity
+
+
 def region_adjacency(labels, K, connectivity=4):
     """Region adjacency graph of int16 labels [B,H,W] (read as uint16) -> RegionGraph(indptr, edge_index, boundary).
 
@@ -78,12 +100,7 @@ def region_adjacency(labels, K, connectivity=4):
     captured in a CUDA graph and raises RuntimeError under capture, before any device work.  All arithmetic is
     integer: the result is exact and the same across runs, batch order, chunking and streams."""
     _tensor("labels", labels, torch.int16, 3)
-    try:
-        connectivity = operator.index(connectivity)
-    except TypeError:
-        raise ValueError("connectivity must be 4 or 8, got %r" % (connectivity,)) from None
-    if connectivity not in (4, 8):
-        raise ValueError("connectivity must be 4 or 8, got %r" % (connectivity,))
+    connectivity = _check_connectivity(connectivity)
     K = _check_K(K)
     B, H, W = (int(v) for v in labels.shape)
     if H * W > MAX_PIXELS:
@@ -144,3 +161,126 @@ def region_adjacency(labels, K, connectivity=4):
             edge_index = torch.cat([p[0] for p in pieces], dim=1)
             boundary = torch.cat([p[1] for p in pieces])
     return RegionGraph(indptr, edge_index, boundary)
+
+
+def boundary_chunk(B, H, W, K, connectivity):
+    """Images per boundary pair selection: as many as fit BOUNDARY_SCRATCH_CAP, at least one."""
+    f = _lib.lib().fslic_b200_boundary_select_scratch_bytes
+    one = int(f(1, H, W, K, connectivity))
+    if one == _NO_SIZE:
+        raise ValueError("an image of %dx%d pixels is too large for boundary statistics" % (H, W))
+    c = max(1, min(B, BOUNDARY_SCRATCH_CAP // max(1, one)))
+    while c > 1:
+        nbytes = int(f(c, H, W, K, connectivity))
+        if nbytes == _NO_SIZE:  # more pixel pairs than one selection takes
+            c //= 2
+            continue
+        if nbytes <= BOUNDARY_SCRATCH_CAP:
+            break
+        c = max(1, min(c - 1, c * BOUNDARY_SCRATCH_CAP // nbytes))
+    return c
+
+
+def boundary_stats(labels, K, graph, values, connectivity=4):
+    """Statistics of pixel maps along the shared boundary of every entry of a region adjacency graph
+    -> BoundaryStats(mean, min, max, count), detached:
+    - mean, min, max float32 [E, C]: one row per entry of graph.edge_index, in its order (PyG's edge_attr layout);
+    - count          int32 [E]: the number of boundary pixel pairs of the entry.
+    labels is a cuda int16 [B,H,W] tensor (read as uint16), values float32 [B,C,H,W] (C >= 1, pool's layout) on the same
+    device.  graph is a RegionGraph (region_adjacency(labels, K, ...)) or any object with indptr of B*K + 1 entries and
+    int64 edge_index [2,E]; only edge_index is read.
+
+    Pixel pairs are region_adjacency's: each pixel (the anchor) with its right and down neighbour, with connectivity 8
+    also the down-right and down-left one.  A pair is a boundary pair when both labels are in [0, K) and differ; its
+    ordinal is anchor_index * D + d, d the direction in that order and D = 2 or 4.  Entry e = (u, v) gets the boundary
+    pairs of image b whose labels are {u % K, v % K} when 0 <= u, v < B*K, u // K == v // K == b and u != v, and none
+    otherwise: both directions of an edge and duplicate entries get identical rows, and entries across images, out of
+    range or with equal endpoints never fault or raise.  The result does not depend on indptr or on the entries' order.
+    - The 2n values of an entry with n pairs, per channel, are values[b, c, anchor] then values[b, c, other] of each
+      pair in increasing ordinal.  count is n: for a graph from region_adjacency with the same labels and connectivity
+      it equals graph.boundary.
+    - mean is their sum in pool's order (dealt to 32 lanes left to right from +0.0, five butterfly steps, lane 0's
+      value) divided by (float)(2n), one correctly rounded division.
+    - min / max follow the total order of non-NaN floats with -0.0 < +0.0; any NaN value makes them NaN (torch.amin /
+      amax).
+    - An entry with no pairs gets count 0 and NaN in mean, min and max, which merge_regions ignores.
+    Each row depends only on labels[b], values[b] and the entry: not on the batch, the chunking, the stream or the run.
+
+    ValueError, before any device work, for: labels that are not a cuda int16 [B,H,W] tensor, values that are not
+    float32 [B,C,H,W] with the labels' B, H, W and C >= 1, K outside [1, 65534], images over 2^29 pixels, connectivity
+    other than 4 or 8, indptr without B*K + 1 entries, edge_index that is not int64 [2,E] (E < 2^31), tensors on
+    different devices.  B, H or W = 0 and E = 0 launch nothing.
+
+    Work runs on the labels' device, on its current stream.  The boundary pair count is data-dependent, so, like
+    region_adjacency, this call reads one int32 back per chunk of images (BOUNDARY_SCRATCH_CAP; a chunk whose pairs need
+    more than the cap to sort is halved and read again, which only maps that are not superpixel maps come near): it
+    cannot be captured in a CUDA graph and raises RuntimeError under capture, before any device work."""
+    _tensor("labels", labels, torch.int16, 3)
+    _tensor("values", values, torch.float32, 4)
+    B, H, W = (int(v) for v in labels.shape)
+    if int(values.shape[0]) != B or tuple(int(v) for v in values.shape[2:]) != (H, W):
+        raise ValueError("values %s do not match labels %s" % (tuple(values.shape), (B, H, W)))
+    C = int(values.shape[1])
+    if C < 1:
+        raise ValueError("values needs at least one channel")
+    connectivity = _check_connectivity(connectivity)
+    K = _check_K(K)
+    if H * W > MAX_PIXELS:
+        raise ValueError("images of %dx%d pixels exceed %d pixels: a boundary count could overflow int32"
+                         % (H, W, MAX_PIXELS))
+    indptr, edge_index = graph.indptr, graph.edge_index
+    if not isinstance(indptr, torch.Tensor) or indptr.numel() != B * K + 1:
+        raise ValueError("graph.indptr must have B*K + 1 = %d entries, got %s" % (
+            B * K + 1, indptr.numel() if isinstance(indptr, torch.Tensor) else type(indptr).__name__))
+    _tensor("graph.edge_index", edge_index, torch.int64, 2)
+    if int(edge_index.shape[0]) != 2:
+        raise ValueError("graph.edge_index must be int64 [2,E], got %s" % (tuple(edge_index.shape),))
+    E = int(edge_index.shape[1])
+    if E > _INT_MAX:
+        raise ValueError("graph.edge_index has %d entries, more than %d: split the graph" % (E, _INT_MAX))
+    for name, x in (("values", values), ("graph.indptr", indptr), ("graph.edge_index", edge_index)):
+        if x.device != labels.device:
+            raise ValueError("%s is on %s, labels on %s" % (name, x.device, labels.device))
+    if labels.device.type != "cuda":
+        raise ValueError("labels is a %s tensor: pass cuda tensors (torch.from_numpy(...).cuda())" % labels.device.type)
+    dev = labels.device
+    with torch.cuda.device(dev):
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("boundary_stats reads its boundary pair count back to the host and cannot be captured in "
+                               "a CUDA graph")
+        if B == 0 or H == 0 or W == 0 or E == 0:  # no pixel pair: every row is absent
+            nan = float("nan")
+            return BoundaryStats(torch.full((E, C), nan, dtype=torch.float32, device=dev),
+                                 torch.full((E, C), nan, dtype=torch.float32, device=dev),
+                                 torch.full((E, C), nan, dtype=torch.float32, device=dev),
+                                 torch.zeros(E, dtype=torch.int32, device=dev))
+        out = BoundaryStats(*(torch.empty((E, C), dtype=torch.float32, device=dev) for _ in range(3)),
+                            torch.empty(E, dtype=torch.int32, device=dev))
+        lab = labels.contiguous()
+        val = values.detach().contiguous()
+        ei = edge_index.contiguous()
+        L = _lib.lib()
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        chunk = boundary_chunk(B, H, W, K, connectivity)
+        work = [(b0, min(chunk, B - b0)) for b0 in range(0, B, chunk)][::-1]
+        first = 1
+        while work:
+            b0, c = work.pop()
+            nbytes = int(L.fslic_b200_boundary_select_scratch_bytes(c, H, W, K, connectivity))
+            select = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            npairs = torch.empty(1, dtype=torch.int32, device=dev)
+            _lib.check(L.fslic_b200_boundary_select_batch(dev.index, c, H, W, K, connectivity, lab[b0].data_ptr(),
+                                                          npairs.data_ptr(), select.data_ptr(), nbytes, stream))
+            pairs = int(npairs.item())  # the host wait: the boundary pair count
+            sbytes = int(L.fslic_b200_boundary_stats_scratch_bytes(pairs, E))
+            if sbytes > BOUNDARY_SCRATCH_CAP and c > 1:  # too many pairs to sort at once: halve the chunk
+                work.extend([(b0 + c // 2, c - c // 2), (b0, c // 2)])
+                continue
+            scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
+            _lib.check(L.fslic_b200_boundary_stats_batch(
+                dev.index, c, H, W, K, C, connectivity, lab[b0].data_ptr(), val[b0].data_ptr(), pairs,
+                select.data_ptr(), nbytes, b0, B * K, E, ei[0].data_ptr(), ei[1].data_ptr(), first,
+                out.mean.data_ptr(), out.min.data_ptr(), out.max.data_ptr(), out.count.data_ptr(), scratch.data_ptr(),
+                sbytes, stream))
+            first = 0
+    return out

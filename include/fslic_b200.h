@@ -346,6 +346,40 @@ int fslic_b200_merge_batch(int device, int batch, int H, int W, int K, const uin
                            double threshold, int num_regions, int32_t* d_region, int32_t* d_num_regions,
                            int16_t* d_out, void* d_scratch, size_t scratch_bytes, void* stream);
 
+/* Boundary statistics of region adjacency edges (boundary.cuh; no counterpart in the reference) over `batch` label
+ * maps d_labels u16[B,H,W] and value maps d_values f32[B,C,H,W].  The pixel pairs are region adjacency's: the right and
+ * down neighbour, with connectivity 8 also the down-right and down-left one; a pair is a boundary pair when both labels
+ * are in [0, K) and differ.  1 <= K <= 65534, H * W <= 2^29.  Two calls per chunk of images, asynchronous on `stream`,
+ * never synchronise: the select writes the number of boundary pairs, the caller reads it back and sizes the stats'
+ * scratch from it, the stats write every graph entry of the chunk's images (DESIGN.md section 4.17).
+ * Scratch bytes of the select (the stats read it too): 4 per pixel pair (2 or 4 per pixel) and the selection's
+ * temporary storage; 256 for no pixel; (size_t)-1 for bad arguments, H * W > 2^29 or more than 2^31 - 1 pixel pairs
+ * (split the batch). */
+size_t fslic_b200_boundary_select_scratch_bytes(int batch, int H, int W, int K, int connectivity);
+/* d_pairs int32[1]: the number of boundary pairs of the call. */
+int fslic_b200_boundary_select_batch(int device, int batch, int H, int W, int K, int connectivity,
+                                     const uint16_t* d_labels, int32_t* d_pairs, void* d_scratch, size_t scratch_bytes,
+                                     void* stream);
+/* Scratch bytes of the stats for `pairs` boundary pairs and `edges` graph entries: 25 per pair, 24 per entry and the
+ * largest temporary storage of the radix sorts and the selection; (size_t)-1 for a negative count or one above
+ * 2^31 - 1. */
+size_t fslic_b200_boundary_stats_scratch_bytes(long long pairs, long long edges);
+/* After a select with the same batch, H, W, K, connectivity, d_labels and d_select_scratch, and `pairs` = its
+ * d_pairs.  The call's images are images [image_base, image_base + batch) of a graph of `nodes` = B_total * K nodes
+ * whose entries are d_src / d_dst int64[E].  Entry e = (u, v) belongs to image b when u // K == v // K == b, both are
+ * in [0, nodes) and u != v; its pairs are image b's boundary pairs whose labels are {u % K, v % K}.  For each entry of
+ * the call's images: d_count int32[E] = the number n of its pairs, and per channel c d_mean / d_min / d_max f32[E,C]
+ * = the mean, min and max of the 2n values of its pairs in ordinal order (anchor, then the other pixel), the sum in
+ * pool's order divided by (float)(2n), min / max under -0.0 < +0.0 and NaN when any value is NaN; NaN and 0 for an
+ * entry with no pairs.  With `first` != 0 every row is first set to NaN and 0, so that entries of no image are
+ * defined: give it to the first call of a batch. */
+int fslic_b200_boundary_stats_batch(int device, int batch, int H, int W, int K, int C, int connectivity,
+                                    const uint16_t* d_labels, const float* d_values, long long pairs,
+                                    const void* d_select_scratch, size_t select_bytes, long long image_base,
+                                    long long nodes, long long edges, const long long* d_src, const long long* d_dst,
+                                    int first, float* d_mean, float* d_min, float* d_max, int32_t* d_count,
+                                    void* d_scratch, size_t scratch_bytes, void* stream);
+
 /* Stage probes for the parity tests (the reference's protected quad_image / assignment,
  * context.h:48-50): copies of the last iterate()'s Lab quad image [B,H,W,4] u8 and pre-CCA
  * labels [B,H,W] u16 into caller device buffers (either may be NULL). */
