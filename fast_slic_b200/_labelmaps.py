@@ -1,0 +1,104 @@
+"""What the batched label-map APIs (pooling, region_graph, groundtruth, geometry, merging, graph_batch) share: their
+argument checks, their limits and the search for how many images one launch takes under a scratch cap."""
+import operator
+
+import torch
+
+MAX_K = 65534
+# Pixels per image: every count over one image fits int32
+MAX_PIXELS = 1 << 29
+# What a *_scratch_bytes entry point returns for arguments no single call takes
+NO_SIZE = 2 ** 64 - 1
+
+
+def tensor(name, x, dtype, ndim):
+    if not isinstance(x, torch.Tensor):
+        raise ValueError("%s must be a cuda tensor (got %s): use torch.from_numpy(...).cuda()" % (name, type(x).__name__))
+    if x.dtype != dtype or x.dim() != ndim:
+        raise ValueError("%s must be a %s tensor with %d dimensions, got %s %s" % (name, dtype, ndim, x.dtype,
+                                                                                 tuple(x.shape)))
+
+
+def check_int(name, v, lo, hi):
+    try:
+        v = operator.index(v)
+    except TypeError:
+        raise ValueError("%s must be an int, got %r" % (name, v)) from None
+    if not lo <= v <= hi:
+        raise ValueError("%s must be in [%d, %d], got %d" % (name, lo, hi, v))
+    return v
+
+
+def check_K(K):
+    return check_int("K", K, 1, MAX_K)
+
+
+def check_connectivity(connectivity):
+    try:
+        connectivity = operator.index(connectivity)
+    except TypeError:
+        raise ValueError("connectivity must be 4 or 8, got %r" % (connectivity,)) from None
+    if connectivity not in (4, 8):
+        raise ValueError("connectivity must be 4 or 8, got %r" % (connectivity,))
+    return connectivity
+
+
+def check_pixels(H, W, reason=""):
+    """Images of at most MAX_PIXELS pixels; `reason` ends the message."""
+    if H * W > MAX_PIXELS:
+        raise ValueError("images of %dx%d pixels exceed %d pixels%s" % (H, W, MAX_PIXELS, reason))
+
+
+def check_features(labels, name, x, ndim):
+    """labels int16 [B,H,W] and x float32 with ndim dimensions, same B (and H, W for ndim 4); returns (B, H, W, C)."""
+    tensor("labels", labels, torch.int16, 3)
+    tensor(name, x, torch.float32, ndim)
+    B, H, W = (int(v) for v in labels.shape)
+    if int(x.shape[0]) != B or (ndim == 4 and tuple(int(v) for v in x.shape[2:]) != (H, W)):
+        raise ValueError("%s %s do not match labels %s" % (name, tuple(x.shape), (B, H, W)))
+    C = int(x.shape[1])
+    if C < 1:
+        raise ValueError("%s needs at least one channel" % name)
+    return B, H, W, C
+
+
+def check_graph(graph, B, K):
+    """graph.indptr of B*K + 1 entries and int64 graph.edge_index [2,E]; returns (edge_index, E)."""
+    indptr, edge_index = graph.indptr, graph.edge_index
+    if not isinstance(indptr, torch.Tensor) or indptr.numel() != B * K + 1:
+        raise ValueError("graph.indptr must have B*K + 1 = %d entries, got %s" % (
+            B * K + 1, indptr.numel() if isinstance(indptr, torch.Tensor) else type(indptr).__name__))
+    tensor("graph.edge_index", edge_index, torch.int64, 2)
+    if int(edge_index.shape[0]) != 2:
+        raise ValueError("graph.edge_index must be int64 [2,E], got %s" % (tuple(edge_index.shape),))
+    return edge_index, int(edge_index.shape[1])
+
+
+def same_device(labels, *named):
+    """Every (name, tensor) of named on the labels' device."""
+    for name, x in named:
+        if x.device != labels.device:
+            raise ValueError("%s is on %s, labels on %s" % (name, x.device, labels.device))
+
+
+def cuda_device(labels, *named):
+    """Every (name, tensor) of named on the labels' device, which must be a cuda device; returns it."""
+    same_device(labels, *named)
+    if labels.device.type != "cuda":
+        raise ValueError("labels is a %s tensor: pass cuda tensors (torch.from_numpy(...).cuda())" % labels.device.type)
+    return labels.device
+
+
+def chunk(size_of, cap, B, limit=None):
+    """Images per launch: as many as size_of(images) bytes of scratch fit in cap, at most B and limit, at least one.
+    A size of NO_SIZE (more images than one launch takes) halves the count."""
+    c = max(1, min(B, B if limit is None else limit, cap // max(1, size_of(1))))
+    while c > 1:
+        nbytes = size_of(c)
+        if nbytes == NO_SIZE:
+            c //= 2
+        elif nbytes <= cap:
+            break
+        else:
+            c = max(1, min(c - 1, c * cap // nbytes))
+    return c

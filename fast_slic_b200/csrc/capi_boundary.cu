@@ -3,22 +3,20 @@
 // caller reads the boundary pair count back between the select and the stats.
 #include <limits.h>
 
-#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_select.cuh>
 #include <thrust/iterator/counting_iterator.h>
 
 #include "boundary.cuh"
 #include "capi_common.h"
-
-#define BOUNDARY_MAX_PIXELS (1LL << 29)  // every pair count of such an image fits int32
+#include "cub_temp.cuh"
 
 static bool boundary_args_ok(int batch, int H, int W, int K, int connectivity) {
-    return batch >= 0 && H >= 0 && W >= 0 && K >= 1 && K <= 65534 && (connectivity == 4 || connectivity == 8);
+    return labels_shape_ok(batch, H, W, K) && (connectivity == 4 || connectivity == 8);
 }
 
 // Pixel-pair slots of a call: D per pixel, -1 when they do not fit one select (int items, uint32 slots)
 static long long boundary_slots(int batch, int H, int W, int connectivity) {
-    if ((long long)H * W > BOUNDARY_MAX_PIXELS) return -1;
+    if ((long long)H * W > MAX_IMAGE_PIXELS) return -1;
     const long long slots = (long long)batch * H * W * (connectivity == 8 ? 4 : 2);
     return slots > INT_MAX ? -1 : slots;
 }
@@ -37,20 +35,29 @@ static size_t boundary_starts_temp_bytes(long long items) {
     return bytes;
 }
 
-static size_t boundary_sort_temp_bytes(long long items) {
-    size_t bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                    (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)items, 0, 64);
-    return bytes;
+// The select's scratch, which the stats read: the selected slots (4 bytes per slot) and the select's temporary storage
+struct SelectScratch {
+    uint32_t* sel;
+    void* temp;
+    size_t temp_bytes, total;
+};
+
+static SelectScratch select_layout(long long slots, const void* base) {
+    SelectScratch s;
+    Carve c(const_cast<void*>(base));
+    s.sel = c.take<uint32_t>((size_t)slots * 4);
+    s.temp_bytes = align_up(boundary_select_temp_bytes(slots), 256);
+    s.temp = c.take<void>(s.temp_bytes);
+    s.total = c.total;
+    return s;
 }
 
-// The select's scratch, which the stats read: the selected slots (4 bytes per slot) and the select's temporary storage
 extern "C" size_t fslic_b200_boundary_select_scratch_bytes(int batch, int H, int W, int K, int connectivity) {
     if (!boundary_args_ok(batch, H, W, K, connectivity)) return (size_t)-1;
     const long long slots = boundary_slots(batch, H, W, connectivity);
     if (slots < 0) return (size_t)-1;
     if (slots == 0) return 256;
-    return align_up((size_t)slots * 4, 256) + align_up(boundary_select_temp_bytes(slots), 256);
+    return select_layout(slots, nullptr).total;
 }
 
 extern "C" int fslic_b200_boundary_select_batch(int device, int batch, int H, int W, int K, int connectivity,
@@ -69,12 +76,11 @@ extern "C" int fslic_b200_boundary_select_batch(int device, int batch, int H, in
     }
     if (!d_labels || !d_scratch) return set_err(FSLIC_EINVAL, "NULL argument");
     if (scratch_bytes < need) return set_err(FSLIC_EINVAL, "scratch too small");
-    uint32_t* sel = static_cast<uint32_t*>(d_scratch);
-    void* temp = static_cast<unsigned char*>(d_scratch) + align_up((size_t)slots * 4, 256);
-    size_t temp_bytes = align_up(boundary_select_temp_bytes(slots), 256);
+    const SelectScratch s = select_layout(slots, d_scratch);
+    size_t temp_bytes = s.temp_bytes;
     const BoundaryPair op{d_labels, (uint32_t)((long long)H * W), (uint32_t)W, (uint32_t)H, (uint32_t)K,
                           connectivity == 8 ? 2 : 1};
-    if (cub::DeviceSelect::If(temp, temp_bytes, thrust::counting_iterator<uint32_t>(0), sel, d_pairs, (int)slots, op,
+    if (cub::DeviceSelect::If(s.temp, temp_bytes, thrust::counting_iterator<uint32_t>(0), s.sel, d_pairs, (int)slots, op,
                               st) != cudaSuccess)
         return set_err(FSLIC_ECUDA, "selection of the boundary pairs failed");
     CK(cudaGetLastError());
@@ -94,31 +100,25 @@ struct BoundaryScratch {
 };
 
 static BoundaryScratch boundary_layout(long long pairs, long long edges, void* base) {
-    BoundaryScratch s{};
-    unsigned char* p = static_cast<unsigned char*>(base);
-    size_t off = 0;
-    auto take = [&](size_t bytes) {
-        void* q = p ? p + off : nullptr;
-        off += align_up(bytes, 256);
-        return q;
-    };
-    s.key = (unsigned long long*)take((size_t)pairs * 8);
-    s.skey = (unsigned long long*)take((size_t)pairs * 8);
-    s.sslot = (uint32_t*)take((size_t)pairs * 4);
-    s.start = (uint32_t*)take((size_t)pairs * 4);
-    s.head = (uint8_t*)take((size_t)pairs);
-    s.ekey = (unsigned long long*)take((size_t)edges * 8);
-    s.sekey = (unsigned long long*)take((size_t)edges * 8);
-    s.eidx = (uint32_t*)take((size_t)edges * 4);
-    s.seidx = (uint32_t*)take((size_t)edges * 4);
-    s.runs = (int*)take(4);
-    size_t temp = boundary_sort_temp_bytes(pairs), t2 = boundary_sort_temp_bytes(edges),
-           t3 = boundary_starts_temp_bytes(pairs);
+    BoundaryScratch s;
+    Carve c(base);
+    s.key = c.take<unsigned long long>((size_t)pairs * 8);
+    s.skey = c.take<unsigned long long>((size_t)pairs * 8);
+    s.sslot = c.take<uint32_t>((size_t)pairs * 4);
+    s.start = c.take<uint32_t>((size_t)pairs * 4);
+    s.head = c.take<uint8_t>((size_t)pairs);
+    s.ekey = c.take<unsigned long long>((size_t)edges * 8);
+    s.sekey = c.take<unsigned long long>((size_t)edges * 8);
+    s.eidx = c.take<uint32_t>((size_t)edges * 4);
+    s.seidx = c.take<uint32_t>((size_t)edges * 4);
+    s.runs = c.take<int>(4);
+    size_t temp = radix_pairs_temp_bytes<unsigned long long, uint32_t>(pairs, 64),
+           t2 = radix_pairs_temp_bytes<unsigned long long, uint32_t>(edges, 64), t3 = boundary_starts_temp_bytes(pairs);
     if (t2 > temp) temp = t2;
     if (t3 > temp) temp = t3;
     s.temp_bytes = align_up(temp, 256);
-    s.temp = take(s.temp_bytes);
-    s.total = off;
+    s.temp = c.take<void>(s.temp_bytes);
+    s.total = c.total;
     return s;
 }
 
@@ -156,7 +156,7 @@ extern "C" int fslic_b200_boundary_stats_batch(int device, int batch, int H, int
         return FSLIC_OK;
     }
     const BoundaryScratch s = boundary_layout(pairs, edges, d_scratch);
-    const uint32_t* sel = static_cast<const uint32_t*>(d_select_scratch);
+    const uint32_t* sel = select_layout(slots, d_select_scratch).sel;
     const uint32_t hw = (uint32_t)((long long)H * W);
     const int shift = connectivity == 8 ? 2 : 1;
     const int bits = 32 + bit_length((unsigned long long)(batch - 1));  // image << 32 | lo << 16 | hi

@@ -581,11 +581,29 @@ static int crf_adopt_stream(fslic_crf* c, void* stream) {
 
 // The graph of `batch` label maps (fslic_b200_get_connectivity_batch's scratch) followed by their counts [batch][K] and
 // neighbour lists [batch][K][12].
+struct PushScratch {
+    void* graph;
+    int32_t* counts;
+    uint32_t* nbrs;
+    size_t graph_bytes, total;
+};
+
+static PushScratch crfdev_push_layout(int K, int batch, void* base) {
+    PushScratch s;
+    Carve c(base);
+    s.graph_bytes = align_up(fslic_b200_connectivity_batch_scratch_bytes(K, batch), 256);
+    s.graph = c.take<void>(s.graph_bytes);
+    s.counts = c.take<int32_t>((size_t)batch * K * 4);
+    s.nbrs = c.take<uint32_t>((size_t)batch * K * CONN_MAX * 4);
+    s.total = c.total;
+    return s;
+}
+
 extern "C" size_t fslic_b200_crfdev_push_scratch_bytes(int K, int batch) {
     const size_t graph = fslic_b200_connectivity_batch_scratch_bytes(K, batch);
     if (graph == (size_t)-1) return graph;
     if (K <= 0 || batch <= 0) return 256;
-    return align_up(graph, 256) + align_up((size_t)batch * K * 4, 256) + align_up((size_t)batch * K * CONN_MAX * 4, 256);
+    return crfdev_push_layout(K, batch, nullptr).total;
 }
 
 // A slot for a device push: from the pool or newly allocated, with room for 12 * N edges (the graph's cap), so the
@@ -660,12 +678,9 @@ static int crfdev_push(fslic_crf* const* owners, int batch, int H, int W, int K,
     }
     const fslic_crf* c0 = owners[0];
     if (!rc) {
-        const size_t graph_bytes = align_up(fslic_b200_connectivity_batch_scratch_bytes(K, batch), 256);
-        unsigned char* p = static_cast<unsigned char*>(d_scratch);
-        int32_t* counts = reinterpret_cast<int32_t*>(p + graph_bytes);
-        uint32_t* nbrs = reinterpret_cast<uint32_t*>(p + graph_bytes + align_up((size_t)batch * K * 4, 256));
-        rc = fslic_b200_get_connectivity_batch(c0->device, batch, H, W, K, d_labels, counts, nbrs, nullptr, d_scratch,
-                                               graph_bytes, st);
+        const PushScratch g = crfdev_push_layout(K, batch, d_scratch);
+        rc = fslic_b200_get_connectivity_batch(c0->device, batch, H, W, K, d_labels, g.counts, g.nbrs, nullptr, g.graph,
+                                               g.graph_bytes, st);
         const long long CN = (long long)c0->C * K;
         const float unbiased = logf((float)c0->C);  // set_unbiased's constant, glibc's logf as on the host path
         const unsigned node_blocks = (unsigned)grid_for(CN > K ? CN : K, c0->device);
@@ -678,8 +693,8 @@ static int crfdev_push(fslic_crf* const* owners, int batch, int H, int W, int K,
             }
             k_feed_nodes<<<dim3(node_blocks, (unsigned)n), 256, 0, st>>>(d_clusters + (size_t)b0 * K, dst, K, c0->C,
                                                                          unbiased);
-            k_feed_csr<<<dim3(1, (unsigned)n), FEED_CSR_THREADS, 0, st>>>(counts + (size_t)b0 * K,
-                                                                          nbrs + (size_t)b0 * K * CONN_MAX, K, dst);
+            k_feed_csr<<<dim3(1, (unsigned)n), FEED_CSR_THREADS, 0, st>>>(g.counts + (size_t)b0 * K,
+                                                                          g.nbrs + (size_t)b0 * K * CONN_MAX, K, dst);
             const cudaError_t e = cudaGetLastError();
             if (e != cudaSuccess) rc = set_err(FSLIC_ECUDA, std::string("feed kernels: ") + cudaGetErrorString(e));
         }

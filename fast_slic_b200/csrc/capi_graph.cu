@@ -3,9 +3,8 @@
 // asynchronous on the caller's stream, never synchronise.  A single-image call is the batch call with batch = 1.
 #include <limits.h>
 
-#include <cub/device/device_radix_sort.cuh>  // library sort for the adjacency graph only (not on the hot path)
-
 #include "capi_common.h"
+#include "cub_temp.cuh"  // library sort for the adjacency graph only (not on the hot path)
 #include "graph.cuh"
 
 // Slots of one image's pair table: a power of two >= max(4096, 32 K)
@@ -14,22 +13,36 @@ static uint32_t conn_table_size(int K) {
     while (t < 32u * (uint32_t)K) t <<= 1;  // a superpixel map has ~3 distinct adjacent pairs per label
     return t;
 }
-static size_t conn_sort_temp_bytes(long long items, int end_bit) {
-    size_t bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                    (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)items, 0, end_bit);
-    return bytes;
-}
-
 // Key and order tables, their sorted copies, the sort's temporary storage (sized for all 64 key bits, an upper bound
 // of what a call sorts) and the per-image overflow flags.
+struct ConnScratch {
+    uint32_t *tkey, *skey;
+    unsigned long long *tord, *sord;
+    void* temp;
+    int* overflow;
+    size_t temp_bytes, total;
+};
+
+static ConnScratch conn_layout(int batch, long long slots, void* base) {
+    ConnScratch s;
+    Carve c(base);
+    s.tkey = c.take<uint32_t>((size_t)slots * 4);
+    s.skey = c.take<uint32_t>((size_t)slots * 4);
+    s.tord = c.take<unsigned long long>((size_t)slots * 8);
+    s.sord = c.take<unsigned long long>((size_t)slots * 8);
+    s.temp_bytes = align_up(radix_pairs_temp_bytes<unsigned long long, uint32_t>(slots, 64), 256);
+    s.temp = c.take<void>(s.temp_bytes);
+    s.overflow = c.take<int>((size_t)batch * 4);
+    s.total = c.total;
+    return s;
+}
+
 extern "C" size_t fslic_b200_connectivity_batch_scratch_bytes(int K, int batch) {
     if (K <= 0 || batch <= 0) return 256;
     if (K > 65535) return (size_t)-1;
     const long long slots = (long long)conn_table_size(K) * batch;
     if (slots > INT_MAX) return (size_t)-1;  // more than one radix sort takes: the call refuses such a batch
-    return align_up((size_t)slots * 4, 256) * 2 + align_up((size_t)slots * 8, 256) * 2 +
-           align_up(conn_sort_temp_bytes(slots, 64), 256) + align_up((size_t)batch * 4, 256);
+    return conn_layout(batch, slots, nullptr).total;
 }
 
 extern "C" int fslic_b200_get_connectivity_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels,
@@ -46,15 +59,9 @@ extern "C" int fslic_b200_get_connectivity_batch(int device, int batch, int H, i
     USE_DEVICE(device);
     if (scratch_bytes < fslic_b200_connectivity_batch_scratch_bytes(K, batch)) return set_err(FSLIC_EINVAL, "scratch too small");
     cudaStream_t st = (cudaStream_t)stream;
-    unsigned char* p = static_cast<unsigned char*>(d_scratch);
-    uint32_t* tkey = reinterpret_cast<uint32_t*>(p); p += align_up((size_t)slots * 4, 256);
-    uint32_t* skey = reinterpret_cast<uint32_t*>(p); p += align_up((size_t)slots * 4, 256);
-    unsigned long long* tord = reinterpret_cast<unsigned long long*>(p); p += align_up((size_t)slots * 8, 256);
-    unsigned long long* sord = reinterpret_cast<unsigned long long*>(p); p += align_up((size_t)slots * 8, 256);
-    size_t temp_bytes = align_up(conn_sort_temp_bytes(slots, 64), 256);
-    if (conn_sort_temp_bytes(slots, bits) > temp_bytes) return set_err(FSLIC_ECUDA, "radix sort temporary storage");
-    void* temp = p; p += temp_bytes;
-    int* overflow = reinterpret_cast<int*>(p);
+    const ConnScratch s = conn_layout(batch, slots, d_scratch);
+    if (radix_pairs_temp_bytes<unsigned long long, uint32_t>(slots, bits) > s.temp_bytes)
+        return set_err(FSLIC_ECUDA, "radix sort temporary storage");
     // the walk's shared memory: u8 counts of the K labels + the staged chunk; opted in once per device for any K
     const int smem = ((K + 15) & ~15) + CONNB_CHUNK * 4, smem_max = 65536 + CONNB_CHUNK * 4;
     static bool walk_smem_set[64] = {};
@@ -62,13 +69,17 @@ extern "C" int fslic_b200_get_connectivity_batch(int device, int batch, int H, i
         CK(cudaFuncSetAttribute(k_connb_walk, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
         if (device >= 0 && device < 64) walk_smem_set[device] = true;
     }
-    k_connb_init<<<(int)grid_for(slots, device), 256, 0, st>>>(tkey, tord, slots, bit_length(T) - 1, obits, batch, overflow);
+    k_connb_init<<<(int)grid_for(slots, device), 256, 0, st>>>(s.tkey, s.tord, slots, bit_length(T) - 1, obits, batch,
+                                                                s.overflow);
     const long n = (long)batch * (H - 1) * (W - 1);
     if (n > 0)
-        k_connb_discover<<<(int)grid_for(n, device), 256, 0, st>>>(d_labels, batch, H, W, K, tkey, tord, T, obits, overflow);
-    if (cub::DeviceRadixSort::SortPairs(temp, temp_bytes, tord, sord, tkey, skey, (int)slots, 0, bits, st) != cudaSuccess)
+        k_connb_discover<<<(int)grid_for(n, device), 256, 0, st>>>(d_labels, batch, H, W, K, s.tkey, s.tord, T, obits,
+                                                                   s.overflow);
+    size_t temp_bytes = s.temp_bytes;
+    if (cub::DeviceRadixSort::SortPairs(s.temp, temp_bytes, s.tord, s.sord, s.tkey, s.skey, (int)slots, 0, bits, st) !=
+        cudaSuccess)
         return set_err(FSLIC_ECUDA, "radix sort of the pair tables failed");
-    k_connb_walk<<<batch, 256, smem, st>>>(skey, T, d_labels, H, W, K, overflow, d_counts, d_neighbors, d_replayed);
+    k_connb_walk<<<batch, 256, smem, st>>>(s.skey, T, d_labels, H, W, K, s.overflow, d_counts, d_neighbors, d_replayed);
     CK(cudaGetLastError());
     return FSLIC_OK;
 }

@@ -7,11 +7,11 @@
 #include "capi_common.h"
 #include "groundtruth.cuh"
 
-#define GT_MAX_PIXELS (1LL << 29)  // every count of such an image fits int32
-#define GT_MAX_BATCH (1 << 17)     // image bits of a key: 17 + 16 label bits + 31 gt bits
+#define GT_MAX_BATCH (1 << 17)  // image bits of a key: 17 + 16 label bits + 31 gt bits
 
-static bool gt_shape_ok(int batch, int H, int W) {
-    return batch >= 0 && H >= 0 && W >= 0 && (long long)H * W <= GT_MAX_PIXELS;
+// K = 1 for the boundary map, which takes any label
+static bool gt_shape_ok(int batch, int H, int W, int K) {
+    return labels_shape_ok(batch, H, W, K) && (long long)H * W <= MAX_IMAGE_PIXELS;
 }
 
 static bool gt_dtype_ok(int dtype) {
@@ -21,23 +21,10 @@ static bool gt_dtype_ok(int dtype) {
 // Bits of the gt field of a key: every valid value of the dtype
 static int gt_bits(int dtype) { return dtype == FSLIC_GT_UINT8 ? 8 : dtype == FSLIC_GT_INT16 ? 15 : 31; }
 
-// A grid of (x, y) blocks of 256 over `per_image` items of each of `batch` images: y = images (at most 65535, the
-// kernels loop over the rest), x = enough blocks for one image, at most about 16 per SM over the whole grid
-static dim3 gt_grid(int batch, long per_image, int device) {
-    int sms = 0;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms <= 0) sms = 1;
-    const unsigned y = batch < 65535 ? (unsigned)batch : 65535u;
-    long x = (per_image + 255) / 256;
-    const long cap = 16L * sms / y;
-    if (x > cap) x = cap;
-    if (x < 1) x = 1;
-    return dim3((unsigned)x, y);
-}
-
 extern "C" int fslic_b200_gt_histogram_batch(int device, int batch, int H, int W, int K, int num_classes, int dtype,
                                              const void* d_classes, const uint16_t* d_labels, int32_t* d_out,
                                              void* stream) {
-    if (!gt_shape_ok(batch, H, W) || K < 1 || K > 65534 || num_classes < 1 || num_classes > 65536 || !gt_dtype_ok(dtype))
+    if (!gt_shape_ok(batch, H, W, K) || num_classes < 1 || num_classes > 65536 || !gt_dtype_ok(dtype))
         return set_err(FSLIC_EINVAL, "bad batch, H, W, K, num_classes or dtype");
     const long hw = (long)H * W, n = (long)batch * hw;
     if (n == 0) return FSLIC_OK;
@@ -83,50 +70,38 @@ static size_t gt_rle_temp_bytes(long long items) {
 // storage of the sort or the encoding, whichever is larger.
 struct GtScratch {
     unsigned long long* key[2];
-    int* cnt;
-    int* nruns;
-    uint32_t* nk;
-    uint32_t* mx;
+    int *cnt, *nruns;
+    uint32_t *nk, *mx;
     unsigned long long* ue;
     uint32_t* bits[3];
     void* temp;
-    size_t temp_bytes;
+    size_t temp_bytes, total;
 };
 
-static size_t gt_layout(int batch, int H, int W, int K, void* base, GtScratch* s) {
+static GtScratch gt_layout(int batch, int H, int W, int K, void* base) {
     const size_t n = (size_t)batch * H * W, nk = (size_t)batch * K, words = (size_t)batch * H * ((W + 31) / 32);
     const size_t sort = gt_sort_temp_bytes((long long)n), rle = gt_rle_temp_bytes((long long)n);
-    const size_t sizes[11] = {align_up(n * 8, 256),  align_up(n * 8, 256),     align_up(n * 4, 256),
-                              256,                   align_up(nk * 4, 256),     align_up(nk * 4, 256),
-                              align_up(nk * 8, 256), align_up(words * 4, 256),  align_up(words * 4, 256),
-                              align_up(words * 4, 256), align_up(sort > rle ? sort : rle, 256)};
-    size_t off[11], total = 0;
-    for (int f = 0; f < 11; f++) {
-        off[f] = total;
-        total += sizes[f];
-    }
-    if (s) {
-        unsigned char* p = static_cast<unsigned char*>(base);
-        s->key[0] = reinterpret_cast<unsigned long long*>(p + off[0]);
-        s->key[1] = reinterpret_cast<unsigned long long*>(p + off[1]);
-        s->cnt = reinterpret_cast<int*>(p + off[2]);
-        s->nruns = reinterpret_cast<int*>(p + off[3]);
-        s->nk = reinterpret_cast<uint32_t*>(p + off[4]);
-        s->mx = reinterpret_cast<uint32_t*>(p + off[5]);
-        s->ue = reinterpret_cast<unsigned long long*>(p + off[6]);
-        for (int f = 0; f < 3; f++) s->bits[f] = reinterpret_cast<uint32_t*>(p + off[7 + f]);
-        s->temp = p + off[10];
-        s->temp_bytes = sizes[10];
-    }
-    return total;
+    GtScratch s;
+    Carve c(base);
+    for (auto& k : s.key) k = c.take<unsigned long long>(n * 8);
+    s.cnt = c.take<int>(n * 4);
+    s.nruns = c.take<int>(4);
+    s.nk = c.take<uint32_t>(nk * 4);
+    s.mx = c.take<uint32_t>(nk * 4);
+    s.ue = c.take<unsigned long long>(nk * 8);
+    for (auto& b : s.bits) b = c.take<uint32_t>(words * 4);
+    s.temp_bytes = align_up(sort > rle ? sort : rle, 256);
+    s.temp = c.take<void>(s.temp_bytes);
+    s.total = c.total;
+    return s;
 }
 
 extern "C" size_t fslic_b200_gt_scores_scratch_bytes(int batch, int H, int W, int K) {
-    if (!gt_shape_ok(batch, H, W) || K < 1 || K > 65534) return (size_t)-1;
+    if (!gt_shape_ok(batch, H, W, K)) return (size_t)-1;
     const long long n = (long long)batch * H * W;
     if (n == 0) return 256;
     if (n > INT_MAX || batch > GT_MAX_BATCH) return (size_t)-1;  // one sort of 64-bit keys: split the batch
-    return gt_layout(batch, H, W, K, nullptr, nullptr);
+    return gt_layout(batch, H, W, K, nullptr).total;
 }
 
 // The two per-pixel passes over the gt of one dtype: the overlap keys into s.key[0] and the three boundary bitmaps
@@ -138,14 +113,14 @@ static void gt_pixel_passes(int batch, int H, int W, int K, int gbits, const voi
     const long hw = (long)H * W, n = (long)batch * hw;
     const int Wd = (W + 31) / 32;
     k_gt_keys<<<(int)grid_for(n, device), 256, 0, st>>>(lab, gt, hw, n, K, gbits, has_ignore, ignore, none, s.key[0]);
-    k_gt_bitmaps<<<gt_grid(batch, (long)H * Wd * 32, device), 256, 0, st>>>(lab, gt, batch, H, W, Wd, has_ignore, ignore,
+    k_gt_bitmaps<<<image_grid(batch, (long)H * Wd * 32, device), 256, 0, st>>>(lab, gt, batch, H, W, Wd, has_ignore, ignore,
                                                                              s.bits[0], s.bits[1], s.bits[2]);
 }
 
 extern "C" int fslic_b200_gt_scores_batch(int device, int batch, int H, int W, int K, int tolerance, int dtype,
                                           const void* d_gt, const uint16_t* d_labels, int has_ignore, long long ignore,
                                           long long* d_out, void* d_scratch, size_t scratch_bytes, void* stream) {
-    if (!gt_shape_ok(batch, H, W) || K < 1 || K > 65534 || tolerance < 0 || tolerance > 32 || !gt_dtype_ok(dtype))
+    if (!gt_shape_ok(batch, H, W, K) || tolerance < 0 || tolerance > 32 || !gt_dtype_ok(dtype))
         return set_err(FSLIC_EINVAL, "bad batch, H, W, K, tolerance or dtype");
     const long hw = (long)H * W, n = (long)batch * hw;
     if (batch == 0) return FSLIC_OK;
@@ -158,8 +133,7 @@ extern "C" int fslic_b200_gt_scores_batch(int device, int batch, int H, int W, i
     const size_t need = fslic_b200_gt_scores_scratch_bytes(batch, H, W, K);
     if (need == (size_t)-1) return set_err(FSLIC_EINVAL, "batch too large for one call: split it");
     if (scratch_bytes < need) return set_err(FSLIC_EINVAL, "scratch too small");
-    GtScratch s;
-    gt_layout(batch, H, W, K, d_scratch, &s);
+    const GtScratch s = gt_layout(batch, H, W, K, d_scratch);
     const int gbits = gt_bits(dtype), bits = bit_length((unsigned long long)(batch - 1)) + 16 + gbits;
     const unsigned long long none = bits >= 64 ? ~0ull : (1ull << bits) - 1;
     const long nk = (long)batch * K;
@@ -178,7 +152,7 @@ extern "C" int fslic_b200_gt_scores_batch(int device, int batch, int H, int W, i
             gt_pixel_passes<int64_t>(batch, H, W, K, gbits, d_gt, d_labels, has_ignore, ignore, none, s, device, st);
     }
     const int Wd = (W + 31) / 32;
-    k_gt_boundary_counts<<<gt_grid(batch, (long)H * Wd, device), 256, 0, st>>>(s.bits[0], s.bits[1], s.bits[2], batch, H,
+    k_gt_boundary_counts<<<image_grid(batch, (long)H * Wd, device), 256, 0, st>>>(s.bits[0], s.bits[1], s.bits[2], batch, H,
                                                                                 Wd, tolerance, d_out);
     // the overlap table: the keys sorted, one run per (image, label, gt)
     cub::DoubleBuffer<unsigned long long> keys(s.key[0], s.key[1]);
@@ -207,7 +181,7 @@ extern "C" int fslic_b200_gt_scores_batch(int device, int batch, int H, int W, i
 
 extern "C" int fslic_b200_gt_boundaries_batch(int device, int batch, int H, int W, const uint16_t* d_labels, uint8_t* d_out,
                                               void* stream) {
-    if (!gt_shape_ok(batch, H, W)) return set_err(FSLIC_EINVAL, "bad batch, H or W");
+    if (!gt_shape_ok(batch, H, W, 1)) return set_err(FSLIC_EINVAL, "bad batch, H or W");
     const long hw = (long)H * W, n = (long)batch * hw;
     if (n == 0) return FSLIC_OK;
     if (!d_labels || !d_out) return set_err(FSLIC_EINVAL, "NULL argument");

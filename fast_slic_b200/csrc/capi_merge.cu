@@ -1,25 +1,21 @@
 // fast_slic_b200/csrc/capi_merge.cu -- the extern "C" entry points of superpixel merging (merge.cuh): single-linkage
 // threshold and region-count cuts of a batch's region adjacency graph.  Stateless (device pointers, caller-provided
 // scratch), asynchronous on the caller's stream, never synchronise and read nothing back: a CUDA graph can capture them.
-#include <cub/device/device_scan.cuh>
 #include <cub/device/device_segmented_radix_sort.cuh>
 
 #include "capi_common.h"
+#include "cub_temp.cuh"
 #include "merge.cuh"
 
 #define MERGE_MAX_NODES (1LL << 30)
 
-static bool merge_shape_ok(int batch, int K) {
-    return batch >= 0 && K >= 1 && K <= 65534 && (long long)batch * K <= MERGE_MAX_NODES;
-}
-
 static size_t merge_sort_temp_bytes(int batch, int K) {
     const int nodes = batch * K;
-    size_t sort = 0, scan = 0;
+    size_t sort = 0;
     cub::DeviceSegmentedRadixSort::SortKeys(nullptr, sort, (const unsigned long long*)nullptr,
                                             (unsigned long long*)nullptr, nodes, batch, (const int*)nullptr,
                                             (const int*)nullptr);
-    cub::DeviceScan::ExclusiveSum(nullptr, scan, (const int*)nullptr, (int*)nullptr, nodes + 1);
+    const size_t scan = exclusive_sum_temp_bytes<int>(nodes + 1);
     return sort > scan ? sort : scan;
 }
 
@@ -34,35 +30,29 @@ struct MergeScratch {
 };
 
 static MergeScratch merge_layout(int batch, int K, void* base) {
-    MergeScratch s{};
+    MergeScratch s;
     const size_t n = (size_t)batch * K;
-    unsigned char* p = static_cast<unsigned char*>(base);
-    size_t off = 0;
-    auto take = [&](size_t bytes) {
-        void* q = p ? p + off : nullptr;
-        off += align_up(bytes, 256);
-        return q;
-    };
-    s.parent = (int*)take(n * 4);
-    s.present = (int*)take(n * 4);
-    s.best = (unsigned long long*)take(n * 8);
-    s.table = (unsigned long long*)take(n * 8);
-    s.sorted = (unsigned long long*)take(n * 8);
-    s.flag = (int*)take((n + 1) * 4);
-    s.pos = (int*)take((n + 1) * 4);
-    s.count = (int*)take((size_t)batch * 4);
-    s.P = (int*)take((size_t)batch * 4);
-    s.seg_begin = (int*)take((size_t)batch * 4);
-    s.seg_end = (int*)take((size_t)batch * 4);
-    s.linked = (int*)take(MERGE_ROUNDS * 4);
+    Carve c(base);
+    s.parent = c.take<int>(n * 4);
+    s.present = c.take<int>(n * 4);
+    s.best = c.take<unsigned long long>(n * 8);
+    s.table = c.take<unsigned long long>(n * 8);
+    s.sorted = c.take<unsigned long long>(n * 8);
+    s.flag = c.take<int>((n + 1) * 4);
+    s.pos = c.take<int>((n + 1) * 4);
+    s.count = c.take<int>((size_t)batch * 4);
+    s.P = c.take<int>((size_t)batch * 4);
+    s.seg_begin = c.take<int>((size_t)batch * 4);
+    s.seg_end = c.take<int>((size_t)batch * 4);
+    s.linked = c.take<int>(MERGE_ROUNDS * 4);
     s.temp_bytes = align_up(merge_sort_temp_bytes(batch, K), 256);
-    s.temp = take(s.temp_bytes);
-    s.total = off;
+    s.temp = c.take<void>(s.temp_bytes);
+    s.total = c.total;
     return s;
 }
 
 extern "C" size_t fslic_b200_merge_scratch_bytes(int batch, int K) {
-    if (!merge_shape_ok(batch, K)) return (size_t)-1;
+    if (batch < 0 || K < 1 || K > MAX_K || (long long)batch * K > MERGE_MAX_NODES) return (size_t)-1;
     if (batch == 0) return 256;
     return merge_layout(batch, K, nullptr).total;
 }
@@ -72,7 +62,8 @@ extern "C" int fslic_b200_merge_batch(int device, int batch, int H, int W, int K
                                       const float* d_weight, int mode, double threshold, int num_regions,
                                       int32_t* d_region, int32_t* d_num_regions, int16_t* d_out, void* d_scratch,
                                       size_t scratch_bytes, void* stream) {
-    if (!merge_shape_ok(batch, K) || H < 0 || W < 0 || edges < 0) return set_err(FSLIC_EINVAL, "bad batch, H, W, K or edges");
+    if (!labels_shape_ok(batch, H, W, K) || (long long)batch * K > MERGE_MAX_NODES || edges < 0)
+        return set_err(FSLIC_EINVAL, "bad batch, H, W, K or edges");
     if (mode != FSLIC_MERGE_THRESHOLD && mode != FSLIC_MERGE_NUM_REGIONS) return set_err(FSLIC_EINVAL, "bad mode");
     if (mode == FSLIC_MERGE_THRESHOLD && threshold != threshold) return set_err(FSLIC_EINVAL, "threshold is NaN");
     if (mode == FSLIC_MERGE_NUM_REGIONS && num_regions < 1) return set_err(FSLIC_EINVAL, "num_regions < 1");

@@ -4,14 +4,13 @@
 #include "capi_common.h"
 #include "props.cuh"
 
-#define PROPS_MAX_PIXELS (1LL << 29)  // with H, W <= 65535 every sum fits int64 and the perimeter int32
-#define PROPS_MAX_SIDE 65535
+#define PROPS_MAX_SIDE 65535  // with MAX_IMAGE_PIXELS every sum fits int64 and the perimeter int32
 
 extern "C" int fslic_b200_props_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels,
                                       int32_t* d_area, int32_t* d_bbox, long long* d_moments, int32_t* d_perimeter,
                                       int32_t* d_border, double* d_centroid, double* d_covariance, void* stream) {
-    if (batch < 0 || H < 0 || W < 0 || H > PROPS_MAX_SIDE || W > PROPS_MAX_SIDE || (long long)H * W > PROPS_MAX_PIXELS ||
-        K < 1 || K > 65534)
+    if (!labels_shape_ok(batch, H, W, K) || H > PROPS_MAX_SIDE || W > PROPS_MAX_SIDE ||
+        (long long)H * W > MAX_IMAGE_PIXELS)
         return set_err(FSLIC_EINVAL, "bad batch, H, W or K");
     if (batch == 0) return FSLIC_OK;
     if (!d_area || !d_bbox || !d_moments || !d_perimeter || !d_border || !d_centroid || !d_covariance ||
@@ -33,17 +32,10 @@ extern "C" int fslic_b200_props_batch(int device, int batch, int H, int W, int K
     }
     const int node_grid = (int)grid_for(nodes, device);
     k_props_init<<<node_grid, 256, 0, st>>>(nodes, o);
-    // tiles: x over one image's tiles, y over images (the kernel loops past 65535), at most about 16 CTAs per SM
-    int sms = 0;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms <= 0) sms = 1;
     const long Wd = (W + 31) / 32;
     const long tiles = (long)ceil_div(H, PROPS_TILE_ROWS) * ((Wd + PROPS_TILE_WORDS - 1) / PROPS_TILE_WORDS);
-    const unsigned gy = batch < 65535 ? (unsigned)batch : 65535u;
-    long gx = tiles;
-    const long cap = 16L * sms / gy;
-    if (gx > cap) gx = cap;
-    if (gx < 1) gx = 1;
-    k_props_tiles<<<dim3((unsigned)gx, gy), 256, 0, st>>>(d_labels, batch, H, W, K, o);
+    // one CTA per tile
+    k_props_tiles<<<image_grid(batch, tiles * 256, device), 256, 0, st>>>(d_labels, batch, H, W, K, o);
     k_props_finish<<<node_grid, 256, 0, st>>>(nodes, o, d_centroid, d_covariance);
     CK(cudaGetLastError());
     return FSLIC_OK;

@@ -3,17 +3,14 @@
 // the edge total back between the count and the fill.
 #include <limits.h>
 
-#include <cub/device/device_radix_sort.cuh>
-#include <cub/device/device_scan.cuh>
-
 #include "capi_common.h"
+#include "cub_temp.cuh"
 #include "rag.cuh"
 
-#define RAG_MAX_PIXELS (1LL << 29)  // every boundary count of such an image fits int32
 #define RAG_MAX_PROBES 512u
 
 static bool rag_args_ok(int batch, int H, int W, int K, int connectivity) {
-    return batch >= 0 && H >= 0 && W >= 0 && K >= 1 && K <= 65534 && (connectivity == 4 || connectivity == 8);
+    return labels_shape_ok(batch, H, W, K) && (connectivity == 4 || connectivity == 8);
 }
 
 // Slots T of one image's pair table (a power of two) and the probe limit.  An image has at most
@@ -42,54 +39,59 @@ static bool rag_table(int H, int W, int K, int connectivity, int exact, uint32_t
     return true;
 }
 
-static size_t rag_scan_temp_bytes(long long items) {
-    size_t bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, bytes, (const long long*)nullptr, (long long*)nullptr, (int)items);
-    return bytes;
-}
-
-static size_t rag_sort_temp_bytes(long long items) {
-    size_t bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                    (const int32_t*)nullptr, (int32_t*)nullptr, (int)items, 0, 64);
-    return bytes;
-}
-
 // The count's scratch, which the fill reads: pair keys and counts (4 bytes each per slot), the degrees and the
 // call-local row offsets (8 bytes each per node, plus one), and the scan's temporary storage.
 struct RagScratch {
-    uint32_t* key;
-    uint32_t* cnt;
+    uint32_t *key, *cnt;
     unsigned long long* deg;
     long long* local;
     void* temp;
-    size_t temp_bytes;
+    size_t temp_bytes, total;
 };
 
-static size_t rag_layout(int batch, uint32_t T, int K, void* base, RagScratch* s) {
+static RagScratch rag_layout(int batch, uint32_t T, int K, const void* base) {
     const size_t slots = (size_t)T * batch, nk1 = (size_t)batch * K + 1;
-    unsigned char* p = static_cast<unsigned char*>(base);
-    const size_t sizes[5] = {align_up(slots * 4, 256), align_up(slots * 4, 256), align_up(nk1 * 8, 256),
-                             align_up(nk1 * 8, 256), align_up(rag_scan_temp_bytes((long long)nk1), 256)};
-    if (s) {
-        s->key = reinterpret_cast<uint32_t*>(p);
-        s->cnt = reinterpret_cast<uint32_t*>(p + sizes[0]);
-        s->deg = reinterpret_cast<unsigned long long*>(p + sizes[0] + sizes[1]);
-        s->local = reinterpret_cast<long long*>(p + sizes[0] + sizes[1] + sizes[2]);
-        s->temp = p + sizes[0] + sizes[1] + sizes[2] + sizes[3];
-        s->temp_bytes = sizes[4];
-    }
-    return sizes[0] + sizes[1] + sizes[2] + sizes[3] + sizes[4];
+    RagScratch s;
+    Carve c(const_cast<void*>(base));
+    s.key = c.take<uint32_t>(slots * 4);
+    s.cnt = c.take<uint32_t>(slots * 4);
+    s.deg = c.take<unsigned long long>(nk1 * 8);
+    s.local = c.take<long long>(nk1 * 8);
+    s.temp_bytes = align_up(exclusive_sum_temp_bytes<long long>((long long)nk1), 256);
+    s.temp = c.take<void>(s.temp_bytes);
+    s.total = c.total;
+    return s;
+}
+
+// The fill's own scratch: edge keys and their sorted copy (8 bytes each per edge), the boundary counts (4 bytes per
+// edge) and the sort's temporary storage (sized for all 64 key bits)
+struct RagFillScratch {
+    unsigned long long *ekey, *skey;
+    int32_t* val;
+    void* temp;
+    size_t temp_bytes, total;
+};
+
+static RagFillScratch rag_fill_layout(long long edges, void* base) {
+    RagFillScratch s;
+    Carve c(base);
+    s.ekey = c.take<unsigned long long>((size_t)edges * 8);
+    s.skey = c.take<unsigned long long>((size_t)edges * 8);
+    s.val = c.take<int32_t>((size_t)edges * 4);
+    s.temp_bytes = align_up(radix_pairs_temp_bytes<unsigned long long, int32_t>(edges, 64), 256);
+    s.temp = c.take<void>(s.temp_bytes);
+    s.total = c.total;
+    return s;
 }
 
 extern "C" size_t fslic_b200_rag_batch_scratch_bytes(int batch, int H, int W, int K, int connectivity, int exact) {
     if (!rag_args_ok(batch, H, W, K, connectivity)) return (size_t)-1;
-    if ((long long)H * W > RAG_MAX_PIXELS) return (size_t)-1;
+    if ((long long)H * W > MAX_IMAGE_PIXELS) return (size_t)-1;
     if ((long long)batch * H * W == 0) return 256;
     if ((long long)batch * K + 1 > INT_MAX) return (size_t)-1;  // one scan and one sort: split the batch
     uint32_t T, probes;
     if (!rag_table(H, W, K, connectivity, exact, &T, &probes)) return (size_t)-1;
-    return rag_layout(batch, T, K, nullptr, nullptr);
+    return rag_layout(batch, T, K, nullptr).total;
 }
 
 extern "C" int fslic_b200_rag_batch_count(int device, int batch, int H, int W, int K, int connectivity, int exact,
@@ -105,8 +107,7 @@ extern "C" int fslic_b200_rag_batch_count(int device, int batch, int H, int W, i
     if (scratch_bytes < need) return set_err(FSLIC_EINVAL, "scratch too small");
     uint32_t T, max_probes;
     rag_table(H, W, K, connectivity, exact, &T, &max_probes);
-    RagScratch s;
-    rag_layout(batch, T, K, d_scratch, &s);
+    const RagScratch s = rag_layout(batch, T, K, d_scratch);
     USE_DEVICE(device);
     cudaStream_t st = (cudaStream_t)stream;
     const long slots = (long)T * batch, nk = (long)batch * K;
@@ -131,11 +132,10 @@ extern "C" int fslic_b200_rag_batch_count(int device, int batch, int H, int W, i
 }
 
 extern "C" size_t fslic_b200_rag_fill_scratch_bytes(int batch, int K, long long edges) {
-    if (batch < 0 || K < 1 || K > 65534 || edges < 0 || edges > INT_MAX || (long long)batch * K + 1 > INT_MAX)
+    if (batch < 0 || K < 1 || K > MAX_K || edges < 0 || edges > INT_MAX || (long long)batch * K + 1 > INT_MAX)
         return (size_t)-1;
     if (edges == 0) return 256;
-    return align_up((size_t)edges * 8, 256) * 2 + align_up((size_t)edges * 4, 256) +
-           align_up(rag_sort_temp_bytes(edges), 256);
+    return rag_fill_layout(edges, nullptr).total;
 }
 
 extern "C" int fslic_b200_rag_batch_fill(int device, int batch, int H, int W, int K, int connectivity, int exact,
@@ -153,23 +153,20 @@ extern "C" int fslic_b200_rag_batch_fill(int device, int batch, int H, int W, in
     if (scratch_bytes < need || fill_bytes < fill_need) return set_err(FSLIC_EINVAL, "scratch too small");
     uint32_t T, max_probes;
     rag_table(H, W, K, connectivity, exact, &T, &max_probes);
-    RagScratch s;
-    rag_layout(batch, T, K, const_cast<void*>(d_scratch), &s);
-    unsigned char* p = static_cast<unsigned char*>(d_fill_scratch);
-    unsigned long long* ekey = reinterpret_cast<unsigned long long*>(p); p += align_up((size_t)edges * 8, 256);
-    unsigned long long* skey = reinterpret_cast<unsigned long long*>(p); p += align_up((size_t)edges * 8, 256);
-    int32_t* val = reinterpret_cast<int32_t*>(p); p += align_up((size_t)edges * 4, 256);
+    const RagScratch s = rag_layout(batch, T, K, d_scratch);
+    const RagFillScratch f = rag_fill_layout(edges, d_fill_scratch);
     const long slots = (long)T * batch, nk = (long)batch * K;
-    size_t temp_bytes = align_up(rag_sort_temp_bytes(edges), 256);
+    size_t temp_bytes = f.temp_bytes;
     const int bits = 16 + bit_length((unsigned long long)(nk - 1));  // row << 16 | target
     USE_DEVICE(device);
     cudaStream_t st = (cudaStream_t)stream;
     CK(cudaMemsetAsync(s.deg, 0, (size_t)nk * 8, st));  // the row cursors
     k_rag_scatter<<<(int)grid_for(slots, device), 256, 0, st>>>(s.key, s.cnt, slots, bit_length(T) - 1, K, s.local, s.deg,
-                                                                ekey, val);
-    if (cub::DeviceRadixSort::SortPairs(p, temp_bytes, ekey, skey, val, d_boundary, (int)edges, 0, bits, st) != cudaSuccess)
+                                                                f.ekey, f.val);
+    if (cub::DeviceRadixSort::SortPairs(f.temp, temp_bytes, f.ekey, f.skey, f.val, d_boundary, (int)edges, 0, bits, st) !=
+        cudaSuccess)
         return set_err(FSLIC_ECUDA, "radix sort of the edges failed");
-    k_rag_emit<<<(int)grid_for(edges, device), 256, 0, st>>>(skey, edges, K, node_base, d_src, d_dst);
+    k_rag_emit<<<(int)grid_for(edges, device), 256, 0, st>>>(f.skey, edges, K, node_base, d_src, d_dst);
     CK(cudaGetLastError());
     return FSLIC_OK;
 }

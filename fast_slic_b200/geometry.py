@@ -17,8 +17,7 @@ import collections
 import torch
 
 from . import _lib
-from .pooling import _check_K, _tensor
-from .region_graph import MAX_PIXELS
+from ._labelmaps import check_K, check_pixels, cuda_device, tensor
 
 # Longest side: with it and MAX_PIXELS every sum fits int64 (sum y^2 of a whole image is at most H W H^2 / 3 < 2^63)
 MAX_SIDE = 65535
@@ -46,16 +45,13 @@ def region_properties(labels, K):
     is not a cuda int16 [B,H,W] tensor, raises ValueError before any device work.  B, H or W = 0 gives zeros without a
     launch.  All kernel arithmetic is integer: image b's result depends only on labels[b], not on the batch, the stream
     or the run."""
-    _tensor("labels", labels, torch.int16, 3)
-    K = _check_K(K)
+    tensor("labels", labels, torch.int16, 3)
+    K = check_K(K)
     B, H, W = (int(v) for v in labels.shape)
     if H > MAX_SIDE or W > MAX_SIDE:
         raise ValueError("images of %dx%d pixels have a side over %d: a moment could overflow int64" % (H, W, MAX_SIDE))
-    if H * W > MAX_PIXELS:
-        raise ValueError("images of %dx%d pixels exceed %d pixels: a moment could overflow int64" % (H, W, MAX_PIXELS))
-    if labels.device.type != "cuda":
-        raise ValueError("labels is a %s tensor: pass cuda tensors (torch.from_numpy(...).cuda())" % labels.device.type)
-    dev = labels.device
+    check_pixels(H, W, ": a moment could overflow int64")
+    dev = cuda_device(labels)
     with torch.cuda.device(dev):
         empty = B == 0 or H == 0 or W == 0
         new = torch.zeros if empty else torch.empty

@@ -11,6 +11,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._labelmaps import chunk
 from .engine import CLUSTER_DTYPE, require_cuda
 
 # Device memory one get_connectivity_batch launch gives its pair tables at most (24 bytes per table slot, 32 slots or
@@ -57,14 +58,8 @@ def _upload(x, is_tensor, dev):
 
 def graph_chunk(K, B):
     """Images per get_connectivity_batch launch: as many as fit GRAPH_SCRATCH_CAP, at least one."""
-    L = _lib.lib()
-    c = max(1, min(B, GRAPH_SCRATCH_CAP // max(1, int(L.fslic_b200_connectivity_batch_scratch_bytes(K, 1)))))
-    while c > 1:
-        nbytes = int(L.fslic_b200_connectivity_batch_scratch_bytes(K, c))
-        if nbytes <= GRAPH_SCRATCH_CAP:
-            break
-        c = max(1, min(c - 1, c * GRAPH_SCRATCH_CAP // nbytes))
-    return c
+    f = _lib.lib().fslic_b200_connectivity_batch_scratch_bytes
+    return chunk(lambda c: f(K, c), GRAPH_SCRATCH_CAP, B)
 
 
 def get_connectivity_batch(K, device, labels, return_replayed=False):

@@ -18,13 +18,11 @@ labels[b] and gt[b] -- not on the batch, its place in it, the chunking, the stre
 describes the kernels.
 """
 import collections
-import operator
 
 import torch
 
 from . import _lib
-from .pooling import _check_K, _devices, _tensor
-from .region_graph import MAX_PIXELS
+from ._labelmaps import NO_SIZE, check_int, check_K, check_pixels, chunk, cuda_device, tensor
 
 # Device memory one scores launch takes at most (about 20.4 bytes per pixel and 16 per superpixel, plus the sort's
 # storage): a batch that needs more runs in chunks of images, with identical results.
@@ -41,20 +39,10 @@ SegmentationScores = collections.namedtuple("SegmentationScores", [
     "asa", "undersegmentation", "boundary_recall", "boundary_precision"])
 
 
-def _int(name, v, lo, hi):
-    try:
-        v = operator.index(v)
-    except TypeError:
-        raise ValueError("%s must be an int, got %r" % (name, v)) from None
-    if not lo <= v <= hi:
-        raise ValueError("%s must be in [%d, %d], got %d" % (name, lo, hi, v))
-    return v
-
-
 def _check(name, gt, labels):
     """labels: int16 [B,H,W]; gt: a [B,H,W] map of a _DTYPES dtype; images of at most MAX_PIXELS pixels.  Returns
     (B, H, W)."""
-    _tensor("labels", labels, torch.int16, 3)
+    tensor("labels", labels, torch.int16, 3)
     if not isinstance(gt, torch.Tensor):
         raise ValueError("%s must be a cuda tensor (got %s): use torch.from_numpy(...).cuda()" % (name, type(gt).__name__))
     if gt.dtype not in _DTYPES:
@@ -62,8 +50,7 @@ def _check(name, gt, labels):
     if tuple(gt.shape) != tuple(labels.shape):
         raise ValueError("%s %s does not match labels %s" % (name, tuple(gt.shape), tuple(labels.shape)))
     B, H, W = (int(v) for v in labels.shape)
-    if H * W > MAX_PIXELS:
-        raise ValueError("images of %dx%d pixels exceed %d pixels: a count could overflow int32" % (H, W, MAX_PIXELS))
+    check_pixels(H, W, ": a count could overflow int32")
     return B, H, W
 
 
@@ -80,9 +67,9 @@ def class_histogram(classes, labels, K, num_classes):
         y = torch.where(h.sum(-1) > 0, h.argmax(-1), -100).reshape(-1)     # [B*K]
     """
     B, H, W = _check("classes", classes, labels)
-    K = _check_K(K)
-    C = _int("num_classes", num_classes, 1, MAX_CLASSES)
-    dev = _devices(labels, "classes", classes)
+    K = check_K(K)
+    C = check_int("num_classes", num_classes, 1, MAX_CLASSES)
+    dev = cuda_device(labels, ("classes", classes))
     with torch.cuda.device(dev):
         out = torch.empty((B, K, C), dtype=torch.int32, device=dev)
         if B == 0 or H == 0 or W == 0:
@@ -97,16 +84,9 @@ def class_histogram(classes, labels, K, num_classes):
 def gt_chunk(B, H, W, K):
     """Images per scores launch: as many as fit GT_SCRATCH_CAP, at least one."""
     f = _lib.lib().fslic_b200_gt_scores_scratch_bytes
-    one = int(f(1, H, W, K))
-    if one == 2 ** 64 - 1:
+    if f(1, H, W, K) == NO_SIZE:
         raise ValueError("an image of %dx%d pixels is too large to score" % (H, W))
-    c = max(1, min(B, _MAX_CHUNK, GT_SCRATCH_CAP // max(1, one)))
-    while c > 1:
-        nbytes = int(f(c, H, W, K))
-        if nbytes <= GT_SCRATCH_CAP:
-            break
-        c = max(1, min(c - 1, c * GT_SCRATCH_CAP // nbytes))
-    return c
+    return chunk(lambda c: f(c, H, W, K), GT_SCRATCH_CAP, B, limit=_MAX_CHUNK)
 
 
 def _ratio(num, den):
@@ -136,10 +116,10 @@ def segmentation_scores(labels, gt, K, tolerance=2, ignore_index=None):
     For several annotations per image, as in BSDS, stack them along B and repeat the labels to match
     (labels.repeat_interleave(A, 0) for A annotations per image)."""
     B, H, W = _check("gt", gt, labels)
-    K = _check_K(K)
-    r = _int("tolerance", tolerance, 0, MAX_TOLERANCE)
-    ignore = None if ignore_index is None else _int("ignore_index", ignore_index, *_INT64)
-    dev = _devices(labels, "gt", gt)
+    K = check_K(K)
+    r = check_int("tolerance", tolerance, 0, MAX_TOLERANCE)
+    ignore = None if ignore_index is None else check_int("ignore_index", ignore_index, *_INT64)
+    dev = cuda_device(labels, ("gt", gt))
     with torch.cuda.device(dev):
         out = torch.zeros((B, 7), dtype=torch.int64, device=dev)
         if B and H and W:
@@ -163,13 +143,10 @@ def boundaries(labels):
     """int16 labels [B,H,W] -> bool [B,H,W]: True at superpixel boundary pixels, those whose right or lower neighbour
     exists and carries another raw label -- a one-sided, 1-pixel-wide outline (what skimage's mark_boundaries draws),
     the same predicate segmentation_scores uses."""
-    _tensor("labels", labels, torch.int16, 3)
+    tensor("labels", labels, torch.int16, 3)
     B, H, W = (int(v) for v in labels.shape)
-    if H * W > MAX_PIXELS:
-        raise ValueError("images of %dx%d pixels exceed %d pixels" % (H, W, MAX_PIXELS))
-    if labels.device.type != "cuda":
-        raise ValueError("labels is a %s tensor: pass cuda tensors (torch.from_numpy(...).cuda())" % labels.device.type)
-    dev = labels.device
+    check_pixels(H, W)
+    dev = cuda_device(labels)
     with torch.cuda.device(dev):
         out = torch.empty((B, H, W), dtype=torch.bool, device=dev)
         if B and H and W:

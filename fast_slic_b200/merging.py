@@ -19,11 +19,10 @@ import operator
 import torch
 
 from . import _lib
-from .pooling import _check_K, _tensor
+from ._labelmaps import NO_SIZE, check_graph, check_K, cuda_device, same_device, tensor
 
 MERGE_THRESHOLD, MERGE_NUM_REGIONS = 0, 1  # FSLIC_MERGE_THRESHOLD, FSLIC_MERGE_NUM_REGIONS
 MAX_NODES = 1 << 30  # B * K: node ids are int32 on the device
-_NO_SIZE = 2 ** 64 - 1
 
 MergeResult = collections.namedtuple("MergeResult", ["labels", "region", "num_regions"])
 
@@ -82,29 +81,18 @@ def merge_regions(labels, K, graph, weights, threshold=None, num_regions=None):
     so a CUDA graph can capture the call.  Scratch comes from torch, sized from B and K.  Once weights are keys all
     arithmetic is integer: the result depends only on the inputs, not on the run, the stream, the batch order or
     splitting the batch."""
-    _tensor("labels", labels, torch.int16, 3)
-    K = _check_K(K)
+    tensor("labels", labels, torch.int16, 3)
+    K = check_K(K)
     B, H, W = (int(v) for v in labels.shape)
     if B * K > MAX_NODES:
         raise ValueError("%d images of K = %d are %d nodes, more than %d: split the batch" % (B, K, B * K, MAX_NODES))
-    indptr, edge_index = graph.indptr, graph.edge_index
-    if not isinstance(indptr, torch.Tensor) or indptr.numel() != B * K + 1:
-        raise ValueError("graph.indptr must have B*K + 1 = %d entries, got %s" % (
-            B * K + 1, indptr.numel() if isinstance(indptr, torch.Tensor) else type(indptr).__name__))
-    _tensor("graph.edge_index", edge_index, torch.int64, 2)
-    if int(edge_index.shape[0]) != 2:
-        raise ValueError("graph.edge_index must be int64 [2,E], got %s" % (tuple(edge_index.shape),))
-    E = int(edge_index.shape[1])
-    _tensor("weights", weights, torch.float32, 1)
+    edge_index, E = check_graph(graph, B, K)
+    tensor("weights", weights, torch.float32, 1)
     if int(weights.shape[0]) != E:
         raise ValueError("weights must be float32 [E] with E = %d, got %s" % (E, tuple(weights.shape)))
-    for name, x in (("graph.indptr", indptr), ("graph.edge_index", edge_index), ("weights", weights)):
-        if x.device != labels.device:
-            raise ValueError("%s is on %s, labels on %s" % (name, x.device, labels.device))
+    same_device(labels, ("graph.indptr", graph.indptr), ("graph.edge_index", edge_index), ("weights", weights))
     mode, t, R = _check_cut(threshold, num_regions)
-    if labels.device.type != "cuda":
-        raise ValueError("labels is a %s tensor: pass cuda tensors (torch.from_numpy(...).cuda())" % labels.device.type)
-    dev = labels.device
+    dev = cuda_device(labels)
     with torch.cuda.device(dev):
         out = MergeResult(torch.empty((B, H, W), dtype=torch.int16, device=dev),
                           torch.empty((B, K), dtype=torch.int32, device=dev),
@@ -113,7 +101,7 @@ def merge_regions(labels, K, graph, weights, threshold=None, num_regions=None):
             return out
         L = _lib.lib()
         nbytes = int(L.fslic_b200_merge_scratch_bytes(B, K))
-        if nbytes == _NO_SIZE:
+        if nbytes == NO_SIZE:
             raise ValueError("no merge of %d images of K = %d" % (B, K))
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         lab = labels.contiguous()

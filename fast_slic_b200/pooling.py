@@ -14,72 +14,23 @@ Cuda tensors only.  Work is enqueued on the labels' device, on its current torch
 labels[b] and features[b] -- not on the batch, the image's place in it, the chunking, the stream or the run
 (DESIGN.md section 4.12 gives the summation order).  pool and unpool are differentiable in features / values.
 """
-import operator
-
 import torch
 from torch.autograd.function import once_differentiable
 
 from . import _lib
+from ._labelmaps import MAX_K, NO_SIZE, check_features, check_K, chunk, cuda_device
 
 # Device memory one pool launch takes for its sort at most (about 16 bytes per pixel plus 8 per superpixel): a batch
 # that needs more runs in chunks of images, with identical results.
 POOL_SCRATCH_CAP = 1 << 30
-MAX_K = 65534
-
-
-def _tensor(name, x, dtype, ndim):
-    if not isinstance(x, torch.Tensor):
-        raise ValueError("%s must be a cuda tensor (got %s): use torch.from_numpy(...).cuda()" % (name, type(x).__name__))
-    if x.dtype != dtype or x.dim() != ndim:
-        raise ValueError("%s must be a %s tensor with %d dimensions, got %s %s" % (name, dtype, ndim, x.dtype,
-                                                                                 tuple(x.shape)))
-
-
-def _devices(labels, name, x):
-    """labels and x on one cuda device; returns it."""
-    if x.device != labels.device:
-        raise ValueError("%s is on %s, labels on %s" % (name, x.device, labels.device))
-    if labels.device.type != "cuda":
-        raise ValueError("labels is a %s tensor: pass cuda tensors (torch.from_numpy(...).cuda())" % labels.device.type)
-    return labels.device
-
-
-def _check_K(K):
-    try:
-        K = operator.index(K)
-    except TypeError:
-        raise ValueError("K must be an int, got %r" % (K,)) from None
-    if not 1 <= K <= MAX_K:
-        raise ValueError("K must be in [1, %d], got %d" % (MAX_K, K))
-    return K
-
-
-def _check_pair(labels, name, x, ndim):
-    """labels int16 [B,H,W] and x float32 with ndim dimensions, same B (and H, W for ndim 4); returns (B, H, W, C)."""
-    _tensor("labels", labels, torch.int16, 3)
-    _tensor(name, x, torch.float32, ndim)
-    B, H, W = (int(v) for v in labels.shape)
-    if int(x.shape[0]) != B or (ndim == 4 and tuple(int(v) for v in x.shape[2:]) != (H, W)):
-        raise ValueError("%s %s do not match labels %s" % (name, tuple(x.shape), (B, H, W)))
-    C = int(x.shape[1])
-    if C < 1:
-        raise ValueError("%s needs at least one channel" % name)
-    return B, H, W, C
 
 
 def pool_chunk(B, H, W, K):
     """Images per pool launch: as many as fit POOL_SCRATCH_CAP, at least one."""
     f = _lib.lib().fslic_b200_pool_batch_scratch_bytes
-    one = int(f(1, H, W, K))
-    if one == 2 ** 64 - 1:
+    if f(1, H, W, K) == NO_SIZE:
         raise ValueError("an image of %dx%d pixels is too large to pool" % (H, W))
-    c = max(1, min(B, 65536, POOL_SCRATCH_CAP // max(1, one)))
-    while c > 1:
-        nbytes = int(f(c, H, W, K))
-        if nbytes <= POOL_SCRATCH_CAP:
-            break
-        c = max(1, min(c - 1, c * POOL_SCRATCH_CAP // nbytes))
-    return c
+    return chunk(lambda c: f(c, H, W, K), POOL_SCRATCH_CAP, B, limit=65536)
 
 
 def _pool(features, labels, K, mean):
@@ -160,9 +111,9 @@ def pool(features, labels, K, reduce="mean", return_counts=False):
     unpool(grad), 0 at pixels of no superpixel."""
     if reduce not in ("mean", "sum"):
         raise ValueError("reduce must be 'mean' or 'sum', got %r" % (reduce,))
-    _check_pair(labels, "features", features, 4)
-    K = _check_K(K)
-    _devices(labels, "features", features)
+    check_features(labels, "features", features, 4)
+    K = check_K(K)
+    cuda_device(labels, ("features", features))
     out, counts = _Pool.apply(features.contiguous(), labels.contiguous(), K, reduce == "mean")
     return (out, counts) if return_counts else out
 
@@ -170,9 +121,9 @@ def pool(features, labels, K, reduce="mean", return_counts=False):
 def unpool(values, labels):
     """float32 values [B,C,K], int16 labels [B,H,W] -> float32 [B,C,H,W]: out[b,c,p] = values[b,c,label(p)], 0.0 where
     the label is outside [0, K).  Differentiable in values: the gradient is pool(grad, labels, K, reduce="sum")."""
-    _check_pair(labels, "values", values, 3)
-    _check_K(int(values.shape[2]))
-    _devices(labels, "values", values)
+    check_features(labels, "values", values, 3)
+    check_K(int(values.shape[2]))
+    cuda_device(labels, ("values", values))
     return _Unpool.apply(values.contiguous(), labels.contiguous())
 
 
@@ -180,11 +131,11 @@ def paint_argmax(q, labels):
     """float32 q [B,C,K] (e.g. SimpleCRFGroup.get_inferred), int16 labels [B,H,W] -> int16 [B,H,W]: the class of each
     pixel's superpixel, the first index of the maximum of q[b, :, label] (a NaN counts as the maximum, as in
     torch.argmax); -1 where the label is outside [0, K).  C <= 32767.  Not differentiable."""
-    B, H, W, C = _check_pair(labels, "q", q, 3)
-    K = _check_K(int(q.shape[2]))
+    B, H, W, C = check_features(labels, "q", q, 3)
+    K = check_K(int(q.shape[2]))
     if C > 32767:
         raise ValueError("paint_argmax gives int16 classes: C must be at most 32767, got %d" % C)
-    dev = _devices(labels, "q", q)
+    dev = cuda_device(labels, ("q", q))
     with torch.cuda.device(dev):
         out = torch.empty((B, H, W), dtype=torch.int16, device=dev)
         if B and H and W:

@@ -16,12 +16,12 @@ No counterpart in the reference: its get_connectivity keeps at most 12 neighbour
 is kept for parity with it.  DESIGN.md sections 4.13 and 4.17 describe the kernels.
 """
 import collections
-import operator
 
 import torch
 
 from . import _lib
-from .pooling import _check_K, _tensor  # the K range of pooling.MAX_K
+from ._labelmaps import (MAX_PIXELS, NO_SIZE, check_connectivity, check_features, check_graph, check_K, check_pixels,
+                         chunk, cuda_device, tensor)
 
 # Device memory the pair tables of one count launch take at most (8 bytes per slot, a power of two >= max(4096, 32 K)
 # slots per image): a batch that needs more runs in chunks of images, with identical results.
@@ -31,10 +31,7 @@ RAG_SCRATCH_CAP = 1 << 30
 # chunk whose boundary pairs need more than this for their sort is split again (only maps that are not superpixel maps,
 # such as noise, have that many).
 BOUNDARY_SCRATCH_CAP = 1 << 30
-# Larger images could have a boundary count above int32
-MAX_PIXELS = 1 << 29
 _INT_MAX = 2 ** 31 - 1
-_NO_SIZE = 2 ** 64 - 1
 
 RegionGraph = collections.namedtuple("RegionGraph", ["indptr", "edge_index", "boundary"])
 BoundaryStats = collections.namedtuple("BoundaryStats", ["mean", "min", "max", "count"])
@@ -43,16 +40,9 @@ BoundaryStats = collections.namedtuple("BoundaryStats", ["mean", "min", "max", "
 def rag_chunk(B, H, W, K, connectivity):
     """Images per count launch: as many as fit RAG_SCRATCH_CAP, at least one."""
     f = _lib.lib().fslic_b200_rag_batch_scratch_bytes
-    one = int(f(1, H, W, K, connectivity, 0))
-    if one == _NO_SIZE:
+    if f(1, H, W, K, connectivity, 0) == NO_SIZE:
         raise ValueError("an image of %dx%d pixels is too large for a region adjacency graph" % (H, W))
-    c = max(1, min(B, RAG_SCRATCH_CAP // max(1, one)))
-    while c > 1:
-        nbytes = int(f(c, H, W, K, connectivity, 0))
-        if nbytes <= RAG_SCRATCH_CAP:
-            break
-        c = max(1, min(c - 1, c * RAG_SCRATCH_CAP // nbytes))
-    return c
+    return chunk(lambda c: f(c, H, W, K, connectivity, 0), RAG_SCRATCH_CAP, B)
 
 
 def _split(b0, flags):
@@ -67,16 +57,6 @@ def _split(b0, flags):
                 runs.append((b0 + i, 1, 1))
             start = i + 1
     return runs
-
-
-def _check_connectivity(connectivity):
-    try:
-        connectivity = operator.index(connectivity)
-    except TypeError:
-        raise ValueError("connectivity must be 4 or 8, got %r" % (connectivity,)) from None
-    if connectivity not in (4, 8):
-        raise ValueError("connectivity must be 4 or 8, got %r" % (connectivity,))
-    return connectivity
 
 
 def region_adjacency(labels, K, connectivity=4):
@@ -99,16 +79,12 @@ def region_adjacency(labels, K, connectivity=4):
     run of images recounted -- only label maps that are not superpixel maps, such as noise, need that).  It cannot be
     captured in a CUDA graph and raises RuntimeError under capture, before any device work.  All arithmetic is
     integer: the result is exact and the same across runs, batch order, chunking and streams."""
-    _tensor("labels", labels, torch.int16, 3)
-    connectivity = _check_connectivity(connectivity)
-    K = _check_K(K)
+    tensor("labels", labels, torch.int16, 3)
+    connectivity = check_connectivity(connectivity)
+    K = check_K(K)
     B, H, W = (int(v) for v in labels.shape)
-    if H * W > MAX_PIXELS:
-        raise ValueError("images of %dx%d pixels exceed %d pixels: a boundary count could overflow int32"
-                         % (H, W, MAX_PIXELS))
-    if labels.device.type != "cuda":
-        raise ValueError("labels is a %s tensor: pass cuda tensors (torch.from_numpy(...).cuda())" % labels.device.type)
-    dev = labels.device
+    check_pixels(H, W, ": a boundary count could overflow int32")
+    dev = cuda_device(labels)
     with torch.cuda.device(dev):
         if torch.cuda.is_current_stream_capturing():
             raise RuntimeError("region_adjacency reads its edge count back to the host and cannot be captured in a "
@@ -127,7 +103,7 @@ def region_adjacency(labels, K, connectivity=4):
         while work:
             b0, c, exact = work.pop()
             nbytes = int(L.fslic_b200_rag_batch_scratch_bytes(c, H, W, K, connectivity, exact))
-            if nbytes == _NO_SIZE:
+            if nbytes == NO_SIZE:
                 raise MemoryError("image %d has too many distinct adjacent label pairs for an exact pair table" % b0)
             scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             info = torch.empty(c + 1, dtype=torch.int64, device=dev)
@@ -166,19 +142,9 @@ def region_adjacency(labels, K, connectivity=4):
 def boundary_chunk(B, H, W, K, connectivity):
     """Images per boundary pair selection: as many as fit BOUNDARY_SCRATCH_CAP, at least one."""
     f = _lib.lib().fslic_b200_boundary_select_scratch_bytes
-    one = int(f(1, H, W, K, connectivity))
-    if one == _NO_SIZE:
+    if f(1, H, W, K, connectivity) == NO_SIZE:
         raise ValueError("an image of %dx%d pixels is too large for boundary statistics" % (H, W))
-    c = max(1, min(B, BOUNDARY_SCRATCH_CAP // max(1, one)))
-    while c > 1:
-        nbytes = int(f(c, H, W, K, connectivity))
-        if nbytes == _NO_SIZE:  # more pixel pairs than one selection takes
-            c //= 2
-            continue
-        if nbytes <= BOUNDARY_SCRATCH_CAP:
-            break
-        c = max(1, min(c - 1, c * BOUNDARY_SCRATCH_CAP // nbytes))
-    return c
+    return chunk(lambda c: f(c, H, W, K, connectivity), BOUNDARY_SCRATCH_CAP, B)
 
 
 def boundary_stats(labels, K, graph, values, connectivity=4):
@@ -215,35 +181,14 @@ def boundary_stats(labels, K, graph, values, connectivity=4):
     region_adjacency, this call reads one int32 back per chunk of images (BOUNDARY_SCRATCH_CAP; a chunk whose pairs need
     more than the cap to sort is halved and read again, which only maps that are not superpixel maps come near): it
     cannot be captured in a CUDA graph and raises RuntimeError under capture, before any device work."""
-    _tensor("labels", labels, torch.int16, 3)
-    _tensor("values", values, torch.float32, 4)
-    B, H, W = (int(v) for v in labels.shape)
-    if int(values.shape[0]) != B or tuple(int(v) for v in values.shape[2:]) != (H, W):
-        raise ValueError("values %s do not match labels %s" % (tuple(values.shape), (B, H, W)))
-    C = int(values.shape[1])
-    if C < 1:
-        raise ValueError("values needs at least one channel")
-    connectivity = _check_connectivity(connectivity)
-    K = _check_K(K)
-    if H * W > MAX_PIXELS:
-        raise ValueError("images of %dx%d pixels exceed %d pixels: a boundary count could overflow int32"
-                         % (H, W, MAX_PIXELS))
-    indptr, edge_index = graph.indptr, graph.edge_index
-    if not isinstance(indptr, torch.Tensor) or indptr.numel() != B * K + 1:
-        raise ValueError("graph.indptr must have B*K + 1 = %d entries, got %s" % (
-            B * K + 1, indptr.numel() if isinstance(indptr, torch.Tensor) else type(indptr).__name__))
-    _tensor("graph.edge_index", edge_index, torch.int64, 2)
-    if int(edge_index.shape[0]) != 2:
-        raise ValueError("graph.edge_index must be int64 [2,E], got %s" % (tuple(edge_index.shape),))
-    E = int(edge_index.shape[1])
+    B, H, W, C = check_features(labels, "values", values, 4)
+    connectivity = check_connectivity(connectivity)
+    K = check_K(K)
+    check_pixels(H, W, ": a boundary count could overflow int32")
+    edge_index, E = check_graph(graph, B, K)
     if E > _INT_MAX:
         raise ValueError("graph.edge_index has %d entries, more than %d: split the graph" % (E, _INT_MAX))
-    for name, x in (("values", values), ("graph.indptr", indptr), ("graph.edge_index", edge_index)):
-        if x.device != labels.device:
-            raise ValueError("%s is on %s, labels on %s" % (name, x.device, labels.device))
-    if labels.device.type != "cuda":
-        raise ValueError("labels is a %s tensor: pass cuda tensors (torch.from_numpy(...).cuda())" % labels.device.type)
-    dev = labels.device
+    dev = cuda_device(labels, ("values", values), ("graph.indptr", graph.indptr), ("graph.edge_index", edge_index))
     with torch.cuda.device(dev):
         if torch.cuda.is_current_stream_capturing():
             raise RuntimeError("boundary_stats reads its boundary pair count back to the host and cannot be captured in "
