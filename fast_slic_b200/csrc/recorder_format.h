@@ -36,7 +36,10 @@ static inline char* put_int(char* p, int v) {
 // quantised distances) skips printf.
 static inline char* put_float(char* p, float v) {
     if (v > -1e6f && v < 1e6f && v == (float)(int)v && !(v == 0.f && signbit(v))) return put_int(p, (int)v);
-    return p + snprintf(p, 32, "%.6g", (double)v);
+    char tmp[32];  // format_report sizes its buffer for kMaxNumber bytes per value: snprintf may not be told more
+    const int n = snprintf(tmp, sizeof(tmp), "%.6g", (double)v);
+    memcpy(p, tmp, (size_t)n);
+    return p + n;
 }
 
 static inline char* put_str(char* p, const char* s) {
@@ -45,8 +48,10 @@ static inline char* put_str(char* p, const char* s) {
     return p + n;
 }
 
-// Longest text of one value: %.6g of a float ("-1.17549e-38", "-nan") or a 32-bit integer, plus a separator.
+// Longest text of one value: %.6g of a float ("-1.17549e-38", "-nan") or a 32-bit integer, plus a separator; of one
+// assignment entry: "65535,".
 static const size_t kMaxNumber = 16;
+static const size_t kMaxLabel = 6;
 static const size_t kMaxCluster = 12 * kMaxNumber + 120;
 
 // The report of `snapshots` snapshots (iterations -1, 0, 1, ...): assignment u16 [snapshots][H*W], min_dists u16 or
@@ -55,7 +60,8 @@ static char* format_report(int H, int W, int K, int snapshots, bool dist_is_floa
                            const void* min_dists, const fslic_cluster* clusters, size_t* len) {
     const size_t N = (size_t)H * W;
     // fixed text of a snapshot: '{"iteration": ', the number, the three array openings, ']}' and ',' -- 78 bytes at most
-    const size_t cap = 128 + (size_t)snapshots * (128 + (size_t)K * kMaxCluster + N * kMaxNumber);
+    // and per pixel one assignment entry and one min_dists value
+    const size_t cap = 128 + (size_t)snapshots * (128 + (size_t)K * kMaxCluster + N * (kMaxLabel + kMaxNumber));
     char* buf = static_cast<char*>(malloc(cap));
     if (!buf) return nullptr;
     char* p = buf;

@@ -120,3 +120,27 @@ def make_slic(case, debug_mode=True):
         s.iterate(image(case), 2)
         s.slic_model.debug_mode = debug_mode
     return s
+
+
+def first_difference(got, want):
+    """Where two reports first differ, for assertion messages."""
+    import json
+    try:
+        g, w = json.loads(got), json.loads(want)
+    except ValueError:  # e.g. "nan" in an LSC report: name the first differing byte instead
+        i = next((i for i, (a, b) in enumerate(zip(got, want)) if a != b), min(len(got), len(want)))
+        return "byte %d: %r vs %r" % (i, got[max(0, i - 40):i + 40], want[max(0, i - 40):i + 40])
+    for key in ("height", "width"):
+        if g[key] != w[key]:
+            return "%s: %r vs %r" % (key, g[key], w[key])
+    if len(g["snapshots"]) != len(w["snapshots"]):
+        return "%d snapshots vs %d" % (len(g["snapshots"]), len(w["snapshots"]))
+    for gs, ws in zip(g["snapshots"], w["snapshots"]):
+        for field in ("iteration", "clusters", "assignment", "min_dists"):
+            if gs[field] != ws[field]:
+                where = ""
+                if isinstance(gs[field], list):
+                    i = next(i for i, (a, b) in enumerate(zip(gs[field], ws[field])) if a != b)
+                    where = " [%d]: %r vs %r" % (i, gs[field][i], ws[field][i])
+                return "snapshot of iteration %d, field %s%s" % (ws["iteration"], field, where)
+    return "same JSON values, different text"

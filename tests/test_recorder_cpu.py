@@ -89,6 +89,20 @@ def test_formatter_max_iter_zero_and_empty():
     assert rep == _python_report(0, 0, z, z, np.zeros((T, 0), CLUSTER_DTYPE))
 
 
+def test_formatter_longest_values():
+    """Every pixel at its longest text: assignment 65535 and a 12-character float min_dist, 19 bytes with their
+    separators, few clusters to pad the buffer.  A buffer sized for one 16-byte value per pixel ran past its end here
+    (an LSC report of a stride-255 call with K = 2: unreached rows keep 65535 and FLT_MAX)."""
+    H, W, T = 40, 50, 3
+    a = np.full((T, H * W), 65535, np.uint16)
+    d = np.full((T, H * W), -1.17549435e-38, np.float32)
+    d[:, ::3] = np.finfo(np.float32).max
+    cl = np.zeros((T, 1), CLUSTER_DTYPE)
+    rep = _lib.format_recorder_report(H, W, a, d, cl)
+    assert rep == _python_report(H, W, a, d, cl)
+    assert len(rep) > T * H * W * 18
+
+
 def test_new_symbols_declared_in_header():
     header = open(os.path.join(ROOT, "include", "fslic_b200.h")).read()
     declared = set(re.findall(r"\b(fslic_b200_\w+)\s*\(", header))

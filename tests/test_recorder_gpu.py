@@ -3,14 +3,13 @@ built) or its pinned SHA-256 digests (tests/golden/recorder_reference_digests.np
 same labels and clusters as untraced, no effect on later untraced calls (graph replay included), batch = singles, host
 entry points refused."""
 import hashlib
-import json
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from recorder_cases import CASES, image, make_slic, reference_report
+from recorder_cases import CASES, first_difference, image, make_slic, reference_report
 
 pytestmark = pytest.mark.gpu
 
@@ -18,29 +17,11 @@ GOLDEN = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golde
 DIGEST = dict(zip(GOLDEN["names"].tolist(), GOLDEN["sha256"].tolist()))
 
 
-def _first_difference(got, want):
-    g, w = json.loads(got), json.loads(want)
-    for key in ("height", "width"):
-        if g[key] != w[key]:
-            return "%s: %r vs %r" % (key, g[key], w[key])
-    if len(g["snapshots"]) != len(w["snapshots"]):
-        return "%d snapshots vs %d" % (len(g["snapshots"]), len(w["snapshots"]))
-    for gs, ws in zip(g["snapshots"], w["snapshots"]):
-        for field in ("iteration", "clusters", "assignment", "min_dists"):
-            if gs[field] != ws[field]:
-                where = ""
-                if isinstance(gs[field], list):
-                    i = next(i for i, (a, b) in enumerate(zip(gs[field], ws[field])) if a != b)
-                    where = " [%d]: %r vs %r" % (i, gs[field][i], ws[field][i])
-                return "snapshot of iteration %d, field %s%s" % (ws["iteration"], field, where)
-    return "same JSON values, different text"
-
-
 def _check_report(case, got):
     from oracle.recorder import RecorderRef
     if RecorderRef.available():
         want = reference_report(case, RecorderRef())
-        assert got == want, case.name + ": " + _first_difference(got, want)
+        assert got == want, case.name + ": " + first_difference(got, want)
     assert hashlib.sha256(got).hexdigest() == DIGEST[case.name], case.name + ": report differs from the reference digest"
 
 
