@@ -12,16 +12,25 @@ as the strength of an edge map between two superpixels, which merging.merge_regi
     s = boundary_stats(labels, K, g, edge_map[:, None])  # [E,1] mean / min / max, [E] pair counts
     m = merge_regions(labels, K, g, s.mean[:, 0], threshold=t)
 
+knn_graph gives the other standard graph over superpixel nodes: each joined to its k nearest superpixels in feature
+space (the MNIST / CIFAR10 superpixel GNN benchmarks use k = 8 over position and mean colour), exact, with ties broken
+by the lower index, in the same node numbering and CSR layout::
+
+    kg = knn_graph(x, 8, present=p.area > 0, symmetric=True)  # x: [B,K,D] node features, p region_properties
+    A = torch.sparse_csr_tensor(kg.indptr, kg.edge_index[1], torch.exp(-kg.distance), (B * K, B * K))
+
 No counterpart in the reference: its get_connectivity keeps at most 12 neighbours per superpixel, in scan order, and
-is kept for parity with it.  DESIGN.md sections 4.13 and 4.17 describe the kernels.
+is kept for parity with it; its get_knn_connectivity has no defined result and raises NotImplementedError here.
+DESIGN.md sections 4.13, 4.17 and 4.18 describe the kernels.
 """
 import collections
 
+import numpy as np
 import torch
 
 from . import _lib
-from ._labelmaps import (MAX_PIXELS, NO_SIZE, check_connectivity, check_features, check_graph, check_K, check_pixels,
-                         chunk, cuda_device, tensor)
+from ._labelmaps import (MAX_PIXELS, NO_SIZE, check_connectivity, check_features, check_graph, check_int, check_K,
+                         check_pixels, chunk, cuda_device, tensor)
 
 # Device memory the pair tables of one count launch take at most (8 bytes per slot, a power of two >= max(4096, 32 K)
 # slots per image): a batch that needs more runs in chunks of images, with identical results.
@@ -31,10 +40,17 @@ RAG_SCRATCH_CAP = 1 << 30
 # chunk whose boundary pairs need more than this for their sort is split again (only maps that are not superpixel maps,
 # such as noise, have that many).
 BOUNDARY_SCRATCH_CAP = 1 << 30
+# Device memory one kNN launch takes at most (about 17 + 4 D + 8 k bytes per node, 72 k more for a symmetric graph):
+# a batch that needs more runs in chunks of images, with identical results.
+KNN_SCRATCH_CAP = 1 << 30
 _INT_MAX = 2 ** 31 - 1
+KNN_MAX_D = 64
+KNN_MAX_NEIGHBORS = 32
+KNN_MAX_NODES = 1 << 30  # B * K
 
 RegionGraph = collections.namedtuple("RegionGraph", ["indptr", "edge_index", "boundary"])
 BoundaryStats = collections.namedtuple("BoundaryStats", ["mean", "min", "max", "count"])
+KnnGraph = collections.namedtuple("KnnGraph", ["indptr", "edge_index", "distance"])
 
 
 def rag_chunk(B, H, W, K, connectivity):
@@ -229,3 +245,98 @@ def boundary_stats(labels, K, graph, values, connectivity=4):
                 sbytes, stream))
             first = 0
     return out
+
+
+def knn_chunk(B, K, D, k, symmetric):
+    """Images per kNN launch: as many as fit KNN_SCRATCH_CAP, at least one."""
+    f = _lib.lib().fslic_b200_knn_scratch_bytes
+    return chunk(lambda c: f(c, K, D, k, int(symmetric)), KNN_SCRATCH_CAP, B)
+
+
+def knn_graph(points, k, present=None, symmetric=False):
+    """k-nearest-neighbour graph of feature points -> KnnGraph(indptr, edge_index, distance).
+
+    points is a cuda float32 [B,K,D] tensor (read detached; a non-contiguous one is made contiguous once); node
+    n = b*K + i is row i of image b and each image is a graph of its own (the block-diagonal numbering of
+    region_adjacency).  present is an optional cuda bool [B,K] on the same device (such as region_properties(...).area
+    > 0); None means every node.  A node is a candidate when it is present and all D coordinates are finite: a node with
+    NaN or +-inf coordinates gets no edges and is no one's neighbour, without raising.
+    - s(i, j), the squared Euclidean distance in float32: t_c = p_i[c] - p_j[c], s = +0.0, s = s + t_c * t_c for
+      c = 0 .. D-1, each operation rounded to nearest on its own (no FMA).  s(i, j) and s(j, i) are the same bits, s is
+      never NaN or -0.0 and is +inf where coordinates are huge; numpy float32 operations in that order give the same.
+    - Node i's neighbours are the first min(k, P_b - 1) other candidates of its image in the order of (s, j), j the
+      local index (ties go to the lower index), P_b being the image's candidate count.  No self loops.
+    - symmetric=False: the directed edges (i -> j), j among i's neighbours.  symmetric=True: those and their reverses,
+      each (source, target) once, which is what PyG's to_undirected makes of the directed graph.
+    Output:
+    - indptr     int64 [B*K + 1]: CSR row offsets; rows of non-candidates are empty.
+    - edge_index int64 [2, E]: (source, target) in global node ids, sorted by source then target, so edge_index[1] is
+      the CSR column array, as in RegionGraph.  Source i -> target j means j is among i's nearest: for PyG's
+      flow="source_to_target" message passing (messages from neighbours to i), pass edge_index.flip(0).
+    - distance   float32 [E]: s of each edge.
+    No edge crosses images.  1 <= K <= 65534, 1 <= D <= 64, 1 <= k <= 32 (an int, not a bool) and B*K <= 2^30;
+    anything else, or points / present of the wrong type, dtype, shape or device, raises ValueError before any device
+    work.  B = 0 gives zero indptr and E = 0.
+
+    Work runs on the points' device, on its current stream.  E is data-dependent, so, like region_adjacency, the call
+    reads the edge total back once per chunk of images (KNN_SCRATCH_CAP); it cannot be captured in a CUDA graph and
+    raises RuntimeError under capture, before any device work.  The result is exact and the same across runs, batch
+    order, chunking and streams: image b's rows depend only on points[b] and present[b]."""
+    tensor("points", points, torch.float32, 3)
+    B, K, D = (int(v) for v in points.shape)
+    K = check_K(K)
+    check_int("D", D, 1, KNN_MAX_D)
+    if B * K > KNN_MAX_NODES:
+        raise ValueError("%d images of K = %d are %d nodes, more than %d: split the batch" % (B, K, B * K, KNN_MAX_NODES))
+    if isinstance(k, (bool, np.bool_)):
+        raise ValueError("k must be an int, got %r" % (k,))
+    k = check_int("k", k, 1, KNN_MAX_NEIGHBORS)
+    symmetric = bool(symmetric)
+    named = []
+    if present is not None:
+        tensor("present", present, torch.bool, 2)
+        if tuple(int(v) for v in present.shape) != (B, K):
+            raise ValueError("present %s do not match points %s" % (tuple(present.shape), (B, K, D)))
+        named.append(("present", present))
+    for name, x in named:
+        if x.device != points.device:
+            raise ValueError("%s is on %s, points on %s" % (name, x.device, points.device))
+    if points.device.type != "cuda":
+        raise ValueError("points is a %s tensor: pass cuda tensors (torch.from_numpy(...).cuda())" % points.device.type)
+    dev = points.device
+    with torch.cuda.device(dev):
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("knn_graph reads its edge count back to the host and cannot be captured in a CUDA graph")
+        indptr = torch.zeros(B * K + 1, dtype=torch.int64, device=dev)
+        if B == 0:
+            return KnnGraph(indptr, torch.empty((2, 0), dtype=torch.int64, device=dev),
+                            torch.empty(0, dtype=torch.float32, device=dev))
+        pts = points.detach().contiguous()
+        pres = present.detach().contiguous().view(torch.uint8) if present is not None else None
+        L = _lib.lib()
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        c = knn_chunk(B, K, D, k, symmetric)
+        nbytes = int(L.fslic_b200_knn_scratch_bytes(c, K, D, k, int(symmetric)))
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        total = torch.empty(1, dtype=torch.int64, device=dev)
+        pieces, edges = [], 0
+        for b0 in range(0, B, c):
+            n = min(c, B - b0)
+            _lib.check(L.fslic_b200_knn_count(dev.index, n, K, D, k, int(symmetric), pts[b0].data_ptr(),
+                                              None if pres is None else pres[b0].data_ptr(), edges,
+                                              indptr[b0 * K:].data_ptr(), total.data_ptr(), scratch.data_ptr(), nbytes,
+                                              stream))
+            e = int(total.item())  # the host wait: the chunk's edge total
+            edge_index = torch.empty((2, e), dtype=torch.int64, device=dev)
+            distance = torch.empty(e, dtype=torch.float32, device=dev)
+            _lib.check(L.fslic_b200_knn_fill(dev.index, n, K, D, k, int(symmetric), b0 * K, e, scratch.data_ptr(),
+                                             nbytes, edge_index[0].data_ptr(), edge_index[1].data_ptr(),
+                                             distance.data_ptr(), stream))
+            pieces.append((edge_index, distance))
+            edges += e
+        if len(pieces) == 1:
+            edge_index, distance = pieces[0]
+        else:
+            edge_index = torch.cat([p[0] for p in pieces], dim=1)
+            distance = torch.cat([p[1] for p in pieces])
+    return KnnGraph(indptr, edge_index, distance)

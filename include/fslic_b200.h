@@ -380,6 +380,29 @@ int fslic_b200_boundary_stats_batch(int device, int batch, int H, int W, int K, 
                                     int first, float* d_mean, float* d_min, float* d_max, int32_t* d_count,
                                     void* d_scratch, size_t scratch_bytes, void* stream);
 
+/* k-nearest-neighbour graphs over feature points (knn.cuh; the reference's get_knn_connectivity has no defined result)
+ * of `batch` images of K points each, d_points f32[B,K,D], node n = b * K + i.  A node is a candidate when
+ * d_present u8[B,K] (NULL: every node) is nonzero and its D coordinates are finite.  s(i, j) = ((+0 + t_0 * t_0) +
+ * t_1 * t_1) + ..., t_c = p_i[c] - p_j[c], every float32 operation rounded on its own.  Node i's neighbours are the first
+ * min(k, P_b - 1) other candidates of its image under the order of (s, j), P_b the image's candidates; with `symmetric`
+ * the edges are those and their reverses, each (source, target) once.  1 <= K <= 65534, 1 <= D <= 64,
+ * 1 <= k <= 32, B * K <= 2^30 and 2 * B * K * k <= 2^31 - 1 per call.  Two calls per chunk of images, asynchronous on
+ * `stream`, never synchronise: the count writes the chunk's row offsets and its edge total, the caller reads the total
+ * back and sizes the outputs, the fill writes the edges (DESIGN.md section 4.18).  Both take the same scratch.
+ * Scratch bytes: per node 17 + 4 * DP + 8 * k (DP: D padded to a power of two >= 4), with `symmetric` 72 * k more, and
+ * the temporary storage of the selection, scan, radix sort and deduplication; (size_t)-1 for arguments out of range. */
+size_t fslic_b200_knn_scratch_bytes(int batch, int K, int D, int k, int symmetric);
+/* d_indptr int64[B*K + 1] = edge_base + the offset of each of the call's rows, the last = edge_base + the total;
+ * d_total int64[1] = the call's edge total. */
+int fslic_b200_knn_count(int device, int batch, int K, int D, int k, int symmetric, const float* d_points,
+                         const uint8_t* d_present, long long edge_base, long long* d_indptr, long long* d_total,
+                         void* d_scratch, size_t scratch_bytes, void* stream);
+/* After a count with the same batch, K, D, k, symmetric and scratch, and `edges` = its total: d_src / d_dst
+ * int64[edges] (node ids + node_base) sorted by source then target, and d_distance f32[edges] = s. */
+int fslic_b200_knn_fill(int device, int batch, int K, int D, int k, int symmetric, long long node_base, long long edges,
+                        const void* d_scratch, size_t scratch_bytes, long long* d_src, long long* d_dst,
+                        float* d_distance, void* stream);
+
 /* Stage probes for the parity tests (the reference's protected quad_image / assignment,
  * context.h:48-50): copies of the last iterate()'s Lab quad image [B,H,W,4] u8 and pre-CCA
  * labels [B,H,W] u16 into caller device buffers (either may be NULL). */
