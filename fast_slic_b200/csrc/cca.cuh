@@ -84,29 +84,6 @@ __device__ __forceinline__ void ccl_union(int* par, int a, int b) {
 // united with shared-memory atomicMin (only where a run overlap starts); every pixel then points at the
 // tile-local root (minimum raster index inside the tile), written as a GLOBAL raster index.
 #define CCL_T 32
-__device__ __forceinline__ int ccl_find_s(const int* par, int x) {
-    int p = par[x];
-    while (p != x) {
-        x = p;
-        p = par[x];
-    }
-    return x;
-}
-__device__ __forceinline__ void ccl_union_s(int* par, int a, int b) {
-    a = ccl_find_s(par, a);
-    b = ccl_find_s(par, b);
-    while (a != b) {
-        if (a < b) {
-            int t = a;
-            a = b;
-            b = t;
-        }
-        const int old = atomicMin(&par[a], b);
-        if (old == a) break;
-        a = ccl_find_s(par, old);
-        b = ccl_find_s(par, b);
-    }
-}
 
 // One WARP per 32 x 32 tile, rows top-down, lane = column.  A run inherits the smallest root among the runs it
 // touches in the row above (a segmented prefix-min by shuffles); shared-memory union-find is only needed
@@ -161,7 +138,7 @@ __global__ void __launch_bounds__(32 * CCL_TW) k_ccl_tile(CcaParams cp, const ui
             const bool conn = (ty > 0) && (up_v == cur);
             const bool need = conn && ((lane == 0) || (left != cur) || (up_left != up_v));
             unsigned cand = 0xffffffffu;
-            if (need) cand = (unsigned)ccl_find_s(s_par, up_root);
+            if (need) cand = (unsigned)ccl_find(s_par, up_root);
             // min over the run: prefix min from the run start, then everyone reads the last lane of the run
             // (REDUX under per-run lane masks is executed one mask at a time -- WARPSYNC.EXCLUSIVE -- and was slower)
             unsigned pm = cand;
@@ -173,7 +150,7 @@ __global__ void __launch_bounds__(32 * CCL_TW) k_ccl_tile(CcaParams cp, const ui
             const unsigned rmin = __shfl_sync(FSLIC_FULL, pm, end);
             const unsigned own = (unsigned)(ty * CCL_T + sl);
             const int root = (int)(rmin < own ? rmin : own);
-            if (need && cand != (unsigned)root) ccl_union_s(s_par, (int)cand, root);  // bridge
+            if (need && cand != (unsigned)root) ccl_union(s_par, (int)cand, root);  // bridge
             s_par[ty * CCL_T + lane] = root;
             __syncwarp();
             up_left = left;
@@ -188,7 +165,7 @@ __global__ void __launch_bounds__(32 * CCL_TW) k_ccl_tile(CcaParams cp, const ui
     uint32_t* aout = area_all + (size_t)b * cp.N + (size_t)(tyb * CCL_T) * cp.W + j;
 #pragma unroll 4
     for (int ty = 0; ty < nrows; ty++) {
-        const int rt = ccl_find_s(s_par, ty * CCL_T + lane);
+        const int rt = ccl_find(s_par, ty * CCL_T + lane);
         const int ri = tyb * CCL_T + (rt >> 5), rj = txb * CCL_T + (rt & 31);
         pout[(size_t)ty * cp.W] = ri * cp.W + rj;
         aout[(size_t)ty * cp.W] = 0;

@@ -1,9 +1,11 @@
-"""Launch decisions and outputs of a fixed matrix of iterate calls, as JSON, for one build of the library:
+"""Launch decisions and outputs of a fixed matrix of iterate and enforce_connectivity calls, as JSON, for one build of
+the library:
 
     python tools/dispatch_record.py path/to/libfslic_b200.so out.json
 
 For every configuration it records launches_last_iterate, dispatch() (with the connectivity stage's decisions),
-graph_counts() and SHA-256 digests of the labels and clusters.  Two builds that make the same launch decisions and
+graph_counts() and SHA-256 digests of the labels and clusters; for the connectivity-only calls the stage's decisions,
+the per-image counters and the label digest.  Two builds that make the same launch decisions and
 compute the same results write identical files, so a host-side change is checked with a diff of two runs (one process
 per library: the binding loads one library per process)."""
 import hashlib
@@ -13,10 +15,12 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+import cca_cases  # noqa: E402
 from bench import synth_images_torch  # noqa: E402
 from fast_slic_b200 import _lib  # noqa: E402
 
@@ -150,6 +154,8 @@ def main(lib_path, out_path):
                 else:
                     eng.iterate_host(im, cl, p, lab)
                 out["%s_call%d" % (name, i)] = record(eng, lab, cl)
+                if collect_timing:  # which of the connectivity stage's sub-sections were timed
+                    out["%s_call%d" % (name, i)]["cca_stage_ms"] = sorted(k for k, v in eng.cca_stage_ms().items() if v > 0)
             eng.close()
 
     for B in (1, 3, 8, 16, 32, 40):
@@ -160,6 +166,27 @@ def main(lib_path, out_path):
     host_run("host_async_b8", 8, is_async=True)
     host_run("host_async_b24", 24, is_async=True)
     host_run("host_async_b2", 2, calls=2, is_async=True)
+
+    # the connectivity stage alone: maps whose K-th largest area is tied (the std::partial_sort replay) beside maps
+    # with fewer candidates than K; one stream (B = 1), the settled images' tail on the side stream (B = 4), sub-batches
+    # of 3 (B = 8), whose counters hold the last sub-batch
+    ties = [cca_cases.random_rect_grid(240, 320, [1, 2], [1, 2, 3], seed) for seed in range(8)]
+    K = cca_cases.k_for(cca_cases.components(ties[0])[2], 1, True, 4)
+    maps = np.stack([ties[i] if i % 2 == 0 else cca_cases.bands(240, 320, [50 + i, 60]) for i in range(8)])
+
+    def cca_run(name, B, sub_batch=None):
+        with Env(**({"FSLIC_CCA_BATCH": str(sub_batch)} if sub_batch else {})):
+            eng = Engine(240, 320, max_batch=B, cca_only=True)
+            lab = torch.from_numpy(maps[:B].view(np.int16)).to(dev)
+            eng.enforce_connectivity(lab, K, 1)
+            torch.cuda.synchronize()
+            out[name] = {"cca": eng.dispatch()["cca"], "labels": digest(lab),
+                         "counters": [eng.cca_counters(i) for i in range(sub_batch or B)]}
+            eng.close()
+
+    cca_run("cca_b1", 1)
+    cca_run("cca_b4", 4)
+    cca_run("cca_b8_sub3", 8, sub_batch=3)
 
     with open(out_path, "w") as f:
         json.dump(out, f, indent=1, sort_keys=True)
