@@ -48,6 +48,7 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_boundary_select_scratch_bytes", "fslic_b200_boundary_select_batch",
     "fslic_b200_boundary_stats_scratch_bytes", "fslic_b200_boundary_stats_batch",
     "fslic_b200_knn_scratch_bytes", "fslic_b200_knn_count", "fslic_b200_knn_fill",
+    "fslic_b200_feature_slic_scratch_bytes", "fslic_b200_feature_slic",
 )
 
 STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity", "iterate")
@@ -162,6 +163,10 @@ def lib():
     L.fslic_b200_knn_scratch_bytes.restype = C.c_size_t
     L.fslic_b200_knn_count.argtypes = [i32, i32, i32, i32, i32, i32, vp, vp, i64, vp, vp, vp, C.c_size_t, vp]
     L.fslic_b200_knn_fill.argtypes = [i32, i32, i32, i32, i32, i32, i64, i64, vp, C.c_size_t, vp, vp, vp, vp]
+    L.fslic_b200_feature_slic_scratch_bytes.argtypes = [i32, i32, i32, i32, i32, i32, i32]
+    L.fslic_b200_feature_slic_scratch_bytes.restype = C.c_size_t
+    L.fslic_b200_feature_slic.argtypes = [i32, i32, i32, i32, i32, i32, C.c_float, i32, i32, vp, vp, vp, vp, vp, vp, vp,
+                                          vp, vp, C.c_size_t, vp]
     L.fslic_b200_assign_kernel_time.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]
     L.fslic_b200_debug_cca_counters.argtypes = [vp, C.POINTER(C.c_int32), i32]
     L.fslic_b200_set_trace.argtypes = [vp, i32]

@@ -6,16 +6,9 @@
 #include "capi_common.h"
 #include "cub_temp.cuh"
 #include "pool.cuh"
+#include "pool_stage.h"
 
-// Keys, pixel indices and their sorted copies (4 bytes each per pixel), the segment bounds (8 bytes per superpixel)
-// and the sort's temporary storage (sized for all 32 key bits).
-struct PoolScratch {
-    uint32_t *key, *skey, *val, *sval, *seg_start, *seg_end;
-    void* temp;
-    size_t temp_bytes, total;
-};
-
-static PoolScratch pool_layout(long long n, long long nk, void* base) {
+PoolScratch pool_layout(long long n, long long nk, void* base) {
     PoolScratch s;
     Carve c(base);
     s.key = c.take<uint32_t>((size_t)n * 4);
@@ -28,6 +21,27 @@ static PoolScratch pool_layout(long long n, long long nk, void* base) {
     s.temp = c.take<void>(s.temp_bytes);
     s.total = c.total;
     return s;
+}
+
+int pool_sorted_segments(const PoolScratch& s, long long n, int batch, int K, int C, long hw, const float* feat,
+                         int mean, float* out, int32_t* counts, int device, cudaStream_t st) {
+    const long nk = (long)batch * K;
+    const int bits = 16 + bit_length((unsigned long long)(batch - 1));
+    CK(cudaMemsetAsync(s.seg_start, 0, (size_t)nk * 4, st));
+    CK(cudaMemsetAsync(s.seg_end, 0, (size_t)nk * 4, st));
+    if (n > 0) {
+        if (radix_pairs_temp_bytes<uint32_t, uint32_t>(n, bits) > s.temp_bytes)
+            return set_err(FSLIC_ECUDA, "radix sort temporary storage");
+        size_t temp_bytes = s.temp_bytes;
+        if (cub::DeviceRadixSort::SortPairs(s.temp, temp_bytes, s.key, s.skey, s.val, s.sval, (int)n, 0, bits, st) !=
+            cudaSuccess)
+            return set_err(FSLIC_ECUDA, "radix sort of the pixel keys failed");
+        k_pool_bounds<<<(int)grid_for(n, device), 256, 0, st>>>(s.skey, n, K, s.seg_start, s.seg_end);
+    }
+    k_pool_segments<<<(unsigned)((nk + 7) / 8), 256, 0, st>>>(s.seg_start, s.seg_end, s.sval, feat, nk, K, C, hw, mean,
+                                                             out, counts);
+    CK(cudaGetLastError());
+    return FSLIC_OK;
 }
 
 extern "C" size_t fslic_b200_pool_batch_scratch_bytes(int batch, int H, int W, int K) {
@@ -52,21 +66,8 @@ extern "C" int fslic_b200_pool_batch(int device, int batch, int H, int W, int C,
     cudaStream_t st = (cudaStream_t)stream;
     const long hw = (long)H * W, nk = (long)batch * K;
     const PoolScratch s = pool_layout(n, nk, d_scratch);
-    const int bits = 16 + bit_length((unsigned long long)(batch - 1));
-    if (radix_pairs_temp_bytes<uint32_t, uint32_t>(n, bits) > s.temp_bytes)
-        return set_err(FSLIC_ECUDA, "radix sort temporary storage");
     k_pool_keys<<<(int)grid_for(n, device), 256, 0, st>>>(d_labels, hw, n, K, s.key, s.val);
-    size_t temp_bytes = s.temp_bytes;
-    if (cub::DeviceRadixSort::SortPairs(s.temp, temp_bytes, s.key, s.skey, s.val, s.sval, (int)n, 0, bits, st) !=
-        cudaSuccess)
-        return set_err(FSLIC_ECUDA, "radix sort of the pixel keys failed");
-    CK(cudaMemsetAsync(s.seg_start, 0, (size_t)nk * 4, st));
-    CK(cudaMemsetAsync(s.seg_end, 0, (size_t)nk * 4, st));
-    k_pool_bounds<<<(int)grid_for(n, device), 256, 0, st>>>(s.skey, n, K, s.seg_start, s.seg_end);
-    k_pool_segments<<<(unsigned)((nk + 7) / 8), 256, 0, st>>>(s.seg_start, s.seg_end, s.sval, d_features, nk, K, C, hw,
-                                                             mean ? 1 : 0, d_out, d_counts);
-    CK(cudaGetLastError());
-    return FSLIC_OK;
+    return pool_sorted_segments(s, n, batch, K, C, hw, d_features, mean ? 1 : 0, d_out, d_counts, device, st);
 }
 
 extern "C" int fslic_b200_pool_unpool_batch(int device, int batch, int H, int W, int C, int K, const uint16_t* d_labels,

@@ -16,6 +16,7 @@
 //   k_prepare2       one thread per cluster over several CTAs per image, the last CTA of an image sorts.
 // Loading and zeroing the accumulated sums stay with each kernel: they use different loads.
 #pragma once
+#include "cellgrid.cuh"
 #include "common.cuh"
 
 struct PrepParams {
@@ -117,52 +118,6 @@ __device__ __forceinline__ CInfo make_record(const fslic_cluster& c, int k, int 
 __device__ __forceinline__ int record_cell(int32_t cyx, const PrepParams& pp) {
     const int cy = (int16_t)(cyx & 0xffff), cx = cyx >> 16;
     return (cy / pp.G) * pp.cellW + (cx / pp.G);
-}
-
-// Step 4: exclusive scan of the cell histogram s_cnt[0, ncnt) by the whole block, between two barriers.  Every thread
-// owns a run of consecutive cells, and one block-wide scan adds up the run totals.  Afterwards s_cnt[c] and cs[c] both
-// hold the first slot of cell c: s_cnt becomes the fill pointer of the scatter, cs is the cell_start the assign kernels
-// read.  s_warp holds one int per warp of the block.
-__device__ __forceinline__ void scan_cells(int* s_cnt, int* s_warp, int* __restrict__ cs, int ncnt, int tid, int nt) {
-    __syncthreads();
-    const int per = (ncnt + nt - 1) / nt;
-    const int c0 = tid * per;
-    int local = 0;
-    for (int u = 0; u < per; u++) {
-        const int c = c0 + u;
-        if (c < ncnt) local += s_cnt[c];
-    }
-    int x = local;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        int y = __shfl_up_sync(FSLIC_FULL, x, o);
-        if ((tid & 31) >= o) x += y;
-    }
-    if ((tid & 31) == 31) s_warp[tid >> 5] = x;
-    __syncthreads();
-    if (tid < 32) {
-        const int nw = nt >> 5;
-        int w = (tid < nw) ? s_warp[tid] : 0;
-        int z = w;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            int y = __shfl_up_sync(FSLIC_FULL, z, o);
-            if (tid >= o) z += y;
-        }
-        if (tid < nw) s_warp[tid] = z - w;
-    }
-    __syncthreads();
-    int run = s_warp[tid >> 5] + x - local;  // exclusive prefix of this thread's first cell
-    for (int u = 0; u < per; u++) {
-        const int c = c0 + u;
-        if (c < ncnt) {
-            const int v = s_cnt[c];
-            s_cnt[c] = run;
-            cs[c] = run;
-            run += v;
-        }
-    }
-    __syncthreads();
 }
 
 // For a grid whose last CTA to arrive finishes the work of all of them: true in every thread of the CTA that takes the

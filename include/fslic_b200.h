@@ -403,6 +403,27 @@ int fslic_b200_knn_fill(int device, int batch, int K, int D, int k, int symmetri
                         const void* d_scratch, size_t scratch_bytes, long long* d_src, long long* d_dst,
                         float* d_distance, void* stream);
 
+/* SLIC over float feature maps (feature_slic.cuh; no counterpart in the reference) of `batch` images d_features
+ * f32[B,C,H,W].  S = (int)(int16_t)sqrt((double)(H * W / K)); seeds on initialize_clusters' grid with the features of
+ * their pixel, or d_init_position f32[B,K,2] (y, x) clamped into the image and d_init_features f32[B,K,C] as given (both
+ * or neither).  Pass t < max_iter assigns the rows i with i % stride == t % stride, then updates; one full assign
+ * follows.  Candidates of pixel (i, j): |i - (int)cy| <= S and |j - (int)cx| <= S; distance d = fc + w2 * (ty*ty +
+ * tx*tx), fc = (((+0 + t_0*t_0) + t_1*t_1) + ..), t_c = f_c - mu_c, ty = i - cy, tx = j - cx, w2 = (compactness / S)^2,
+ * every float32 operation rounded on its own; the winner is the smallest (bits(d) << 32 | k), a NaN distance having
+ * the bits 0x7fffffff; a pixel without a candidate keeps its label (initially 0xffff).  Update over the pass rows: n
+ * members, cy = (float)((double)sum_i / n), cx likewise, mu = pool's mean (fslic_b200_pool_batch's summation order); a
+ * cluster with n = 0 keeps its centre and features.  Outputs: d_labels u16[B,H,W] before connectivity enforcement,
+ * d_position f32[B,K,2], d_centroids f32[B,K,C], d_count i32[B,K] (n of the last update, 0 when max_iter = 0), and,
+ * unless NULL, d_overflow i32[max_iter + 1]: the tiles of each pass that overflowed to the per-pixel assign kernel.
+ * 1 <= C <= 1024, 1 <= K <= min(65534, H * W), H, W <= 32767, H * W <= 2^29, B * K <= 2^30, 1 <= stride <= 255,
+ * max_iter >= 0, compactness finite and > 0; B * H * W <= 2^31 - 1 and B <= 65535 per call.  Asynchronous on `stream`,
+ * never synchronises (DESIGN.md section 4.19).  Scratch bytes: (size_t)-1 for arguments out of range. */
+size_t fslic_b200_feature_slic_scratch_bytes(int batch, int H, int W, int C, int K, int stride, int max_iter);
+int fslic_b200_feature_slic(int device, int batch, int H, int W, int C, int K, float compactness, int stride,
+                            int max_iter, const float* d_features, const float* d_init_position,
+                            const float* d_init_features, uint16_t* d_labels, float* d_position, float* d_centroids,
+                            int32_t* d_count, int32_t* d_overflow, void* d_scratch, size_t scratch_bytes, void* stream);
+
 /* Stage probes for the parity tests (the reference's protected quad_image / assignment,
  * context.h:48-50): copies of the last iterate()'s Lab quad image [B,H,W,4] u8 and pre-CCA
  * labels [B,H,W] u16 into caller device buffers (either may be NULL). */
