@@ -49,6 +49,9 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_boundary_stats_scratch_bytes", "fslic_b200_boundary_stats_batch",
     "fslic_b200_knn_scratch_bytes", "fslic_b200_knn_count", "fslic_b200_knn_fill",
     "fslic_b200_feature_slic_scratch_bytes", "fslic_b200_feature_slic",
+    "fslic_b200_soft_assign", "fslic_b200_soft_assign_backward", "fslic_b200_soft_pool",
+    "fslic_b200_soft_pool_backward", "fslic_b200_soft_unpool", "fslic_b200_soft_unpool_backward",
+    "fslic_b200_soft_labels",
 )
 
 STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity", "iterate")
@@ -167,6 +170,14 @@ def lib():
     L.fslic_b200_feature_slic_scratch_bytes.restype = C.c_size_t
     L.fslic_b200_feature_slic.argtypes = [i32, i32, i32, i32, i32, i32, C.c_float, i32, i32, vp, vp, vp, vp, vp, vp, vp,
                                           vp, vp, C.c_size_t, vp]
+    soft = [i32] * 7  # device, batch, H, W, C, nh, nw
+    L.fslic_b200_soft_assign.argtypes = soft + [vp] * 4
+    L.fslic_b200_soft_assign_backward.argtypes = soft + [vp] * 8
+    L.fslic_b200_soft_pool.argtypes = soft + [vp] * 5
+    L.fslic_b200_soft_pool_backward.argtypes = soft + [vp] * 10
+    L.fslic_b200_soft_unpool.argtypes = soft + [vp] * 4
+    L.fslic_b200_soft_unpool_backward.argtypes = soft + [vp] * 6
+    L.fslic_b200_soft_labels.argtypes = [i32] * 6 + [vp] * 3
     L.fslic_b200_assign_kernel_time.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]
     L.fslic_b200_debug_cca_counters.argtypes = [vp, C.POINTER(C.c_int32), i32]
     L.fslic_b200_set_trace.argtypes = [vp, i32]

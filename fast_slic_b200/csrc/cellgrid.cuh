@@ -1,7 +1,13 @@
 // fast_slic_b200/csrc/cellgrid.cuh -- device helpers of the seed grid and the cell grid that the u16 path
-// (lab.cuh, prepare.cuh) and feature_slic.cuh share.  No kernels: any translation unit may include it.
+// (lab.cuh, prepare.cuh), feature_slic.cuh and soft_slic.cuh share.  No kernels: any translation unit may include it.
 #pragma once
 #include "common.cuh"
+
+// One channel's term of the squared feature distance: fc + (x - mu)^2, each operation rounded on its own
+__device__ __forceinline__ float fs_acc(float fc, float x, float mu) {
+    const float t = __fsub_rn(x, mu);
+    return __fadd_rn(fc, __fmul_rn(t, t));
+}
 
 // The seed centre (cy, cx) of cluster k on the grid of BaseContext::initialize_clusters (context.cpp:43-86): walks
 // the row bands to find the band / column its index falls in (O(sqrt K)).  Also the seeds of feature_slic.cuh.

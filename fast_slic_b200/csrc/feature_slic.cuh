@@ -28,12 +28,6 @@ struct FsParams {
     int tiles_x, tiles;  // tiles per pass row band and per image
 };
 
-// One channel's term of the feature distance
-__device__ __forceinline__ float fs_acc(float fc, float x, float mu) {
-    const float t = __fsub_rn(x, mu);
-    return __fadd_rn(fc, __fmul_rn(t, t));
-}
-
 // The packed key of candidate k of pixel (i, j) from its feature distance fc
 __device__ __forceinline__ unsigned long long fs_key(float fc, int i, int j, float cy, float cx, float w2, int k) {
     const float ty = __fsub_rn((float)i, cy), tx = __fsub_rn((float)j, cx);

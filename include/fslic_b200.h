@@ -424,6 +424,43 @@ int fslic_b200_feature_slic(int device, int batch, int H, int W, int C, int K, f
                             const float* d_init_features, uint16_t* d_labels, float* d_position, float* d_centroids,
                             int32_t* d_count, int32_t* d_overflow, void* d_scratch, size_t scratch_bytes, void* stream);
 
+/* Differentiable soft SLIC (soft_slic.cuh; no counterpart in the reference; DESIGN.md section 4.20) over a grid of nh x
+ * nw cells, K = nh * nw: pixel (i, j) is in cell (i*nh / H, j*nw / W), and its 9 slots n = (da+1)*3 + (db+1) are the
+ * cells (a+da, b+db), invalid outside the grid (value +0.0, in no sum).  Per-pixel maps f32[B,C,H,W], associations and
+ * their gradients f32[B,9,H,W], per-cell maps f32[B,C,K], weights Z f32[B,K].  Every float32 operation is rounded on its
+ * own in a fixed order: sums over slots in n order, over channels in c order, over a cell's block (the pixels with the
+ * cell in a valid slot, a rectangle) in pool's lane order, all from +0.0.  1 <= nh <= H, 1 <= nw <= W, K <= 65534,
+ * H * W <= 2^29, B * K <= 2^30, C >= 1.  Asynchronous on `stream`, never synchronise; batch 0 does nothing.
+ *   soft_assign: q_n = e_n / sum e, e_n = expf(m - d_n) (glibc's), d_n = sum_c (f_c - mu_{k(n)c})^2, m = fminf of d
+ *   soft_assign_backward (d_gd: a f32[B,9,H,W] temporary; either gradient may be NULL): gd_n = q_n * (t - g_n),
+ *     t = sum_n q_n g_n; gF_c = 2 * sum_n gd_n (f_c - mu_{k(n)c}); gmu_kc = -2 * block sum of gd (f_c - mu_kc)
+ *   soft_pool: A = block sum of q v, Z = block sum of q, M = A / Z where Z != 0, else 0
+ *   soft_pool_backward (d_grad_sums f32[B,C,K] and d_grad_weights f32[B,K] temporaries; the last two outputs may be
+ *     NULL): gA = gM / Z, gZ = -sum_c gA M (both 0 where Z == 0); gV_c = sum_n q_n gA_{k(n)c};
+ *     gQ_n = sum_c gA_{k(n)c} v_c + gZ_{k(n)}
+ *   soft_unpool: out_c = sum_n q_n M_{k(n)c}
+ *   soft_unpool_backward (either output may be NULL): gM = block sum of q g; gQ_n = sum_c g_c M_{k(n)c}
+ *   soft_labels: the cell of each pixel's first largest q over its valid slots, a NaN counting as the maximum */
+int fslic_b200_soft_assign(int device, int batch, int H, int W, int C, int nh, int nw, const float* d_features,
+                           const float* d_centroids, float* d_assoc, void* stream);
+int fslic_b200_soft_assign_backward(int device, int batch, int H, int W, int C, int nh, int nw,
+                                    const float* d_features, const float* d_centroids, const float* d_assoc,
+                                    const float* d_grad_assoc, float* d_gd, float* d_grad_features,
+                                    float* d_grad_centroids, void* stream);
+int fslic_b200_soft_pool(int device, int batch, int H, int W, int C, int nh, int nw, const float* d_values,
+                         const float* d_assoc, float* d_means, float* d_weights, void* stream);
+int fslic_b200_soft_pool_backward(int device, int batch, int H, int W, int C, int nh, int nw, const float* d_values,
+                                  const float* d_assoc, const float* d_means, const float* d_weights,
+                                  const float* d_grad_means, float* d_grad_sums, float* d_grad_weights,
+                                  float* d_grad_values, float* d_grad_assoc, void* stream);
+int fslic_b200_soft_unpool(int device, int batch, int H, int W, int C, int nh, int nw, const float* d_values,
+                           const float* d_assoc, float* d_out, void* stream);
+int fslic_b200_soft_unpool_backward(int device, int batch, int H, int W, int C, int nh, int nw, const float* d_values,
+                                    const float* d_assoc, const float* d_grad_out, float* d_grad_values,
+                                    float* d_grad_assoc, void* stream);
+int fslic_b200_soft_labels(int device, int batch, int H, int W, int nh, int nw, const float* d_assoc,
+                           uint16_t* d_labels, void* stream);
+
 /* Stage probes for the parity tests (the reference's protected quad_image / assignment,
  * context.h:48-50): copies of the last iterate()'s Lab quad image [B,H,W,4] u8 and pre-CCA
  * labels [B,H,W] u16 into caller device buffers (either may be NULL). */
