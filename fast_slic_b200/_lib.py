@@ -52,6 +52,9 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_soft_assign", "fslic_b200_soft_assign_backward", "fslic_b200_soft_pool",
     "fslic_b200_soft_pool_backward", "fslic_b200_soft_unpool", "fslic_b200_soft_unpool_backward",
     "fslic_b200_soft_labels",
+    "fslic_b200_mp_gather", "fslic_b200_mp_gather_backward_scratch_bytes", "fslic_b200_mp_gather_backward",
+    "fslic_b200_mp_softmax", "fslic_b200_mp_softmax_backward", "fslic_b200_mp_aggregate",
+    "fslic_b200_mp_aggregate_backward_scratch_bytes", "fslic_b200_mp_aggregate_backward",
 )
 
 STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity", "iterate")
@@ -178,6 +181,16 @@ def lib():
     L.fslic_b200_soft_unpool.argtypes = soft + [vp] * 4
     L.fslic_b200_soft_unpool_backward.argtypes = soft + [vp] * 6
     L.fslic_b200_soft_labels.argtypes = [i32] * 6 + [vp] * 3
+    L.fslic_b200_mp_gather.argtypes = [i32, i64, i64, i32, i32] + [vp] * 5
+    L.fslic_b200_mp_gather_backward_scratch_bytes.argtypes = [i64, i64]
+    L.fslic_b200_mp_gather_backward_scratch_bytes.restype = C.c_size_t
+    L.fslic_b200_mp_gather_backward.argtypes = [i32, i64, i64, i32, i32] + [vp] * 5 + [C.c_size_t, vp]
+    L.fslic_b200_mp_softmax.argtypes = [i32, i64, i64, i32] + [vp] * 5
+    L.fslic_b200_mp_softmax_backward.argtypes = [i32, i64, i64, i32] + [vp] * 6
+    L.fslic_b200_mp_aggregate.argtypes = [i32, i64, i64, i32, i32, i32] + [vp] * 8
+    L.fslic_b200_mp_aggregate_backward_scratch_bytes.argtypes = [i64, i64, i32, i32]
+    L.fslic_b200_mp_aggregate_backward_scratch_bytes.restype = C.c_size_t
+    L.fslic_b200_mp_aggregate_backward.argtypes = [i32, i64, i64, i32, i32, i32] + [vp] * 10 + [C.c_size_t, vp]
     L.fslic_b200_assign_kernel_time.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]
     L.fslic_b200_debug_cca_counters.argtypes = [vp, C.POINTER(C.c_int32), i32]
     L.fslic_b200_set_trace.argtypes = [vp, i32]

@@ -461,6 +461,47 @@ int fslic_b200_soft_unpool_backward(int device, int batch, int H, int W, int C, 
 int fslic_b200_soft_labels(int device, int batch, int H, int W, int nh, int nw, const float* d_assoc,
                            uint16_t* d_labels, void* stream);
 
+/* Message passing over superpixel graphs (message_passing.cuh; no counterpart in the reference; DESIGN.md section
+ * 4.21).  A graph is d_indptr int64 [N+1] (CSR offsets) and d_targets int64 [E] (edge_index[1]): the row of entry e is
+ * the node n with indptr[n] <= e < indptr[n+1], its target t_e = targets[e].  An entry with t_e outside [0, N) is no
+ * edge: it takes part in nothing and receives no gradient.  Every float operation is separately rounded, in a fixed
+ * order: row sums over a node's entries in increasing e, column sums over a node's in-entries (the entries targeting
+ * it) in increasing e, both from +0.0; no float atomics.  0 <= N, E <= 2^31 - 1, C >= 1, H >= 1 divides C.  Node maps
+ * [N,C], entry maps [E,C], weights and scores [E,H]; head h owns channels [h*C/H, (h+1)*C/H).  Asynchronous on
+ * `stream`, never synchronise.
+ *   mp_gather (end 0: target, 1: source): out[e] = x[t_e] or x[row(e)], +0.0 for no edge
+ *   mp_gather_backward: end 1: grad_x[n] = row sum of g[e]; end 0: column sum of g[e] (d_scratch as its
+ *     *_scratch_bytes says; unused for end 1)
+ *   mp_softmax: per row and head, m = the maximum (NaN wins; -0.0 < +0.0), y_e = expf(s_e - m) (glibc's), Z = row sum
+ *     of y, out_e = y_e / Z
+ *   mp_softmax_backward: dot = row sum of out_e * g_e; grad_e = out_e * (g_e - dot)
+ *   mp_aggregate (reduce 0: sum, 1: mean, 2: max; d_weight [E,H] or NULL): term w[e,h] * x[t_e,c] (x[t_e,c] without a
+ *     weight); sum: the row sum; mean: sum / (float)deg, d_deg int32 [N] receives deg; max: the first maximal term
+ *     (NaN wins; -0.0 < +0.0), d_amax int32 [N,C] receives its entry (-1 for none); an empty row gives +0.0
+ *   mp_aggregate_backward (d_deg for mean, d_amax for max, as the forward wrote them; either output may be NULL):
+ *     G = g, or g / (float)deg for mean; grad_x[t,c] = column sum of w[e,h] * G[row(e),c]; grad_w[e,h] = the sum of
+ *     G[row(e),c] * x[t_e,c] over head h's channels in pool's lane order; for max only the terms an entry won */
+int fslic_b200_mp_gather(int device, long long N, long long E, int C, int end, const long long* d_indptr,
+                         const long long* d_targets, const float* d_x, float* d_out, void* stream);
+size_t fslic_b200_mp_gather_backward_scratch_bytes(long long N, long long E);
+int fslic_b200_mp_gather_backward(int device, long long N, long long E, int C, int end, const long long* d_indptr,
+                                  const long long* d_targets, const float* d_grad_out, float* d_grad_x, void* d_scratch,
+                                  size_t scratch_bytes, void* stream);
+int fslic_b200_mp_softmax(int device, long long N, long long E, int H, const long long* d_indptr,
+                          const long long* d_targets, const float* d_scores, float* d_out, void* stream);
+int fslic_b200_mp_softmax_backward(int device, long long N, long long E, int H, const long long* d_indptr,
+                                   const long long* d_targets, const float* d_out, const float* d_grad_out,
+                                   float* d_grad_scores, void* stream);
+int fslic_b200_mp_aggregate(int device, long long N, long long E, int C, int H, int reduce, const long long* d_indptr,
+                            const long long* d_targets, const float* d_x, const float* d_weight, float* d_out,
+                            int32_t* d_deg, int32_t* d_amax, void* stream);
+size_t fslic_b200_mp_aggregate_backward_scratch_bytes(long long N, long long E, int C, int reduce);
+int fslic_b200_mp_aggregate_backward(int device, long long N, long long E, int C, int H, int reduce,
+                                     const long long* d_indptr, const long long* d_targets, const float* d_x,
+                                     const float* d_weight, const int32_t* d_deg, const int32_t* d_amax,
+                                     const float* d_grad_out, float* d_grad_x, float* d_grad_weight, void* d_scratch,
+                                     size_t scratch_bytes, void* stream);
+
 /* Stage probes for the parity tests (the reference's protected quad_image / assignment,
  * context.h:48-50): copies of the last iterate()'s Lab quad image [B,H,W,4] u8 and pre-CCA
  * labels [B,H,W] u16 into caller device buffers (either may be NULL). */
