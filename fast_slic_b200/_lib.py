@@ -55,6 +55,8 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_mp_gather", "fslic_b200_mp_gather_backward_scratch_bytes", "fslic_b200_mp_gather_backward",
     "fslic_b200_mp_softmax", "fslic_b200_mp_softmax_backward", "fslic_b200_mp_aggregate",
     "fslic_b200_mp_aggregate_backward_scratch_bytes", "fslic_b200_mp_aggregate_backward",
+    "fslic_b200_sv_enforce_scratch_bytes", "fslic_b200_sv_enforce", "fslic_b200_sv_slic_scratch_bytes",
+    "fslic_b200_sv_slic",
 )
 
 STAGE_NAMES = ("cielab_conversion", "assign", "update", "full_assign", "enforce_connectivity", "iterate")
@@ -191,6 +193,12 @@ def lib():
     L.fslic_b200_mp_aggregate_backward_scratch_bytes.argtypes = [i64, i64, i32, i32]
     L.fslic_b200_mp_aggregate_backward_scratch_bytes.restype = C.c_size_t
     L.fslic_b200_mp_aggregate_backward.argtypes = [i32, i64, i64, i32, i32, i32] + [vp] * 10 + [C.c_size_t, vp]
+    L.fslic_b200_sv_enforce_scratch_bytes.argtypes = [i32] * 4
+    L.fslic_b200_sv_enforce_scratch_bytes.restype = C.c_size_t
+    L.fslic_b200_sv_enforce.argtypes = [i32] * 7 + [vp] * 3 + [C.c_size_t, vp]
+    L.fslic_b200_sv_slic_scratch_bytes.argtypes = [i32] * 10
+    L.fslic_b200_sv_slic_scratch_bytes.restype = C.c_size_t
+    L.fslic_b200_sv_slic.argtypes = [i32] * 9 + [C.c_float] * 3 + [i32] * 3 + [vp] * 7 + [C.c_size_t, vp]
     L.fslic_b200_assign_kernel_time.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int)]
     L.fslic_b200_debug_cca_counters.argtypes = [vp, C.POINTER(C.c_int32), i32]
     L.fslic_b200_set_trace.argtypes = [vp, i32]

@@ -9,6 +9,13 @@ __device__ __forceinline__ float fs_acc(float fc, float x, float mu) {
     return __fadd_rn(fc, __fmul_rn(t, t));
 }
 
+// The packed assign key of candidate k at distance d: bits(d) << 32 | k, a NaN distance having the bits 0x7fffffff, so
+// the smallest key is the nearest candidate with ties to the lower k (feature_slic.cuh, supervoxel.cuh)
+__device__ __forceinline__ unsigned long long dist_key(float d, int k) {
+    const uint32_t bits = isnan(d) ? 0x7fffffffu : __float_as_uint(d);
+    return (unsigned long long)bits << 32 | (uint32_t)k;
+}
+
 // The seed centre (cy, cx) of cluster k on the grid of BaseContext::initialize_clusters (context.cpp:43-86): walks
 // the row bands to find the band / column its index falls in (O(sqrt K)).  Also the seeds of feature_slic.cuh.
 __device__ __forceinline__ void init_grid_centre(int k, int H, int W, int K, int& cy_out, int& cx_out) {

@@ -31,9 +31,7 @@ struct FsParams {
 // The packed key of candidate k of pixel (i, j) from its feature distance fc
 __device__ __forceinline__ unsigned long long fs_key(float fc, int i, int j, float cy, float cx, float w2, int k) {
     const float ty = __fsub_rn((float)i, cy), tx = __fsub_rn((float)j, cx);
-    const float d = __fadd_rn(fc, __fmul_rn(w2, __fadd_rn(__fmul_rn(ty, ty), __fmul_rn(tx, tx))));
-    const uint32_t bits = isnan(d) ? 0x7fffffffu : __float_as_uint(d);
-    return (unsigned long long)bits << 32 | (uint32_t)k;
+    return dist_key(__fadd_rn(fc, __fmul_rn(w2, __fadd_rn(__fmul_rn(ty, ty), __fmul_rn(tx, tx)))), k);
 }
 
 __device__ __forceinline__ bool fs_in_window(int i, int j, float cy, float cx, int S) {

@@ -675,6 +675,37 @@ int fslic_b200_crfdev_group_get_inferred(fslic_crf* const* crfs, int n, float* d
  * host wait per stream the members are on. */
 int fslic_b200_crfgroup_pop_frame(fslic_crf* const* crfs, int n, int* times_out);
 
+/* Supervoxels (supervoxel.cuh, sv_cca.cuh; no counterpart in the reference; DESIGN.md section 4.22).
+ * Connectivity enforcement of `batch` label volumes d_labels u16[B,D,H,W] into d_out i16[B,D,H,W] (d_out may be
+ * d_labels): components are the 6-connected sets of equal labels, numbered by leader (smallest raster index) order;
+ * those of area >= min_size are candidates, of more than K the K first by (area descending, leader ascending) are
+ * kept and take 0, 1, .. in leader order; component 0 takes 0 if not kept; every other component takes the label of
+ * the component of its leader's predecessor voxel (leader - 1 if x > 0, else - W if y > 0, else - H*W).  1 <= K <=
+ * 65534, min_size >= 0, D, H, W <= 32767, D*H*W <= 2^29; B*D*H*W < 2^31 - 1 and B <= 65535 per call.  Scratch bytes:
+ * (size_t)-1 for arguments out of range. */
+size_t fslic_b200_sv_enforce_scratch_bytes(int batch, int D, int H, int W);
+int fslic_b200_sv_enforce(int device, int batch, int D, int H, int W, int K, int min_size, const uint16_t* d_labels,
+                          int16_t* d_out, void* d_scratch, size_t scratch_bytes, void* stream);
+/* SLIC over `batch` volumes d_volumes f32[B,C,D,H,W] on an nd x nh x nw seed grid (K = nd*nh*nw <= 65534, 1 <= n_a <=
+ * L_a): seed k = (iz*nh + iy)*nw + ix at the integer centre (lo + hi - 1) / 2 of its cell [i*L/n, (i+1)*L/n) on every
+ * axis with that voxel's features.  Pass t < max_iter assigns the voxels of the rows y % stride == t % stride of every
+ * slice, then updates; one full assign follows, then the enforcement above with min_size.  Candidates of voxel v:
+ * |v_a - (int)c_a| <= R_a = ceil(L_a / n_a) on every axis; distance d = fc + ((w2z*(tz*tz) + w2y*(ty*ty)) +
+ * w2x*(tx*tx)), fc = (((+0 + t_0*t_0) + t_1*t_1) + ..), t_c = f_c - mu_c, t_a = v_a - c_a, every float32 operation
+ * rounded on its own; the winner is the smallest (bits(d) << 32 | k), a NaN distance having the bits 0x7fffffff; a
+ * voxel without a candidate keeps its label (initially 0xffff).  Update: c_a = (float)((double)sum v_a / n), mu =
+ * pool's mean over the pass voxels; a cluster with n = 0 keeps both.  Outputs: d_labels i16[B,D,H,W] after
+ * enforcement, d_position f32[B,K,3] (z, y, x), d_centroids f32[B,K,C], d_count i32[B,K] (n of the last update, 0 when
+ * max_iter = 0), and unless NULL d_overflow i32[max_iter + 1]: the tiles of each pass that went to the per-voxel
+ * assign kernel.  1 <= C <= 1024, B*K <= 2^30, 1 <= stride <= 255, max_iter >= 0, w2 finite and >= 0; per call as
+ * fslic_b200_sv_enforce.  Asynchronous on `stream`, never synchronises. */
+size_t fslic_b200_sv_slic_scratch_bytes(int batch, int D, int H, int W, int C, int nd, int nh, int nw, int stride,
+                                        int max_iter);
+int fslic_b200_sv_slic(int device, int batch, int D, int H, int W, int C, int nd, int nh, int nw, float w2z, float w2y,
+                       float w2x, int stride, int max_iter, int min_size, const float* d_volumes, int16_t* d_labels,
+                       float* d_position, float* d_centroids, int32_t* d_count, int32_t* d_overflow, void* d_scratch,
+                       size_t scratch_bytes, void* stream);
+
 /* glibc's logf as the device feed evaluates it (fast_slic_b200/csrc/glibc_logf.cuh), like the expf pair above. */
 int fslic_b200_debug_logf_host(uint32_t first, long long n, float* h_out);
 int fslic_b200_debug_logf_device(int device, uint32_t first, long long n, float* d_out, void* stream);
