@@ -1,5 +1,6 @@
-"""What the batched label-map APIs (pooling, region_graph, groundtruth, geometry, merging, graph_batch) share: their
-argument checks, their limits and the search for how many images one launch takes under a scratch cap."""
+"""What the batched label-map APIs (pooling, region_graph, groundtruth, geometry, merging, graph_batch) and SLIC over
+float data (feature_slic, supervoxels) share: their argument checks, their limits and the search for how many images one
+launch takes under a scratch cap."""
 import operator
 
 import torch
@@ -9,6 +10,11 @@ MAX_K = 65534
 MAX_PIXELS = 1 << 29
 # What a *_scratch_bytes entry point returns for arguments no single call takes
 NO_SIZE = 2 ** 64 - 1
+# SLIC over float data (csrc/capi_float_slic.cu): channels, side, B*K and subsample stride
+FLOAT_SLIC_MAX_C = 1024
+FLOAT_SLIC_MAX_SIDE = 32767
+FLOAT_SLIC_MAX_NODES = 1 << 30
+FLOAT_SLIC_MAX_STRIDE = 255
 
 
 def tensor(name, x, dtype, ndim):
@@ -27,6 +33,12 @@ def check_int(name, v, lo, hi):
     if not lo <= v <= hi:
         raise ValueError("%s must be in [%d, %d], got %d" % (name, lo, hi, v))
     return v
+
+
+def check_number(name, v):
+    if isinstance(v, bool) or not isinstance(v, (int, float)) and not hasattr(v, "__float__"):
+        raise ValueError("%s must be a number, got %r" % (name, v))
+    return float(v)
 
 
 def check_K(K):
@@ -102,3 +114,30 @@ def chunk(size_of, cap, B, limit=None):
         else:
             c = max(1, min(c - 1, c * cap // nbytes))
     return c
+
+
+def slic_pass_tiles(shape, tile, max_iter, subsample_stride):
+    """Tiles per image of every assign pass of SLIC over float data: max_iter strided passes over the rows (the
+    second-last axis of shape, (H, W) or (D, H, W)), then the full one, with tiles of the shape `tile` (same axes)."""
+    rows = shape[-2]
+    out = []
+    for t in range(max_iter + 1):
+        r, s = (t % subsample_stride, subsample_stride) if t < max_iter else (0, 1)
+        npr = (rows - 1 - r) // s + 1 if r < rows else 0
+        n = 1
+        for a, (L, T) in enumerate(zip(shape, tile)):
+            n *= -(-(npr if a == len(shape) - 2 else L) // T)
+        out.append(n)
+    return out
+
+
+def slic_dispatch(run, x, max_iter, subsample_stride, tile):
+    """run(max_iter, overflow) on x [B,C,*shape] with a record of the assign kernels it ran (synchronises): (result,
+    [(tiles, overflowed)] per pass), the tiles of the pass over the whole batch and how many of them overflowed the
+    tile kernel's candidate list and went to the per-pixel kernel."""
+    B = int(x.shape[0]) if isinstance(x, torch.Tensor) else 0
+    max_iter = operator.index(max_iter)
+    overflow = torch.zeros((max(B, 1), max_iter + 1), dtype=torch.int32, device=x.device)
+    r = run(max_iter, overflow)
+    tiles = slic_pass_tiles(tuple(int(v) for v in x.shape[2:]), tile, max_iter, subsample_stride)
+    return r, [(B * t, int(o)) for t, o in zip(tiles, overflow.sum(0).tolist())]

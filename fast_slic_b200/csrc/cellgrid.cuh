@@ -1,5 +1,5 @@
 // fast_slic_b200/csrc/cellgrid.cuh -- device helpers of the seed grid and the cell grid that the u16 path
-// (lab.cuh, prepare.cuh), feature_slic.cuh and soft_slic.cuh share.  No kernels: any translation unit may include it.
+// (lab.cuh, prepare.cuh), float_slic.cuh and soft_slic.cuh share.  No kernels: any translation unit may include it.
 #pragma once
 #include "common.cuh"
 
@@ -10,14 +10,14 @@ __device__ __forceinline__ float fs_acc(float fc, float x, float mu) {
 }
 
 // The packed assign key of candidate k at distance d: bits(d) << 32 | k, a NaN distance having the bits 0x7fffffff, so
-// the smallest key is the nearest candidate with ties to the lower k (feature_slic.cuh, supervoxel.cuh)
+// the smallest key is the nearest candidate with ties to the lower k (float_slic.cuh)
 __device__ __forceinline__ unsigned long long dist_key(float d, int k) {
     const uint32_t bits = isnan(d) ? 0x7fffffffu : __float_as_uint(d);
     return (unsigned long long)bits << 32 | (uint32_t)k;
 }
 
 // The seed centre (cy, cx) of cluster k on the grid of BaseContext::initialize_clusters (context.cpp:43-86): walks
-// the row bands to find the band / column its index falls in (O(sqrt K)).  Also the seeds of feature_slic.cuh.
+// the row bands to find the band / column its index falls in (O(sqrt K)).  Also k_fs_seed's (float_slic.cuh).
 __device__ __forceinline__ void init_grid_centre(int k, int H, int W, int K, int& cy_out, int& cx_out) {
     const int n_y = (int)sqrt((double)K);
     const int base_n = K / n_y, remainder = K % n_y;

@@ -1,4 +1,4 @@
-"""SLIC over float feature maps on the GPU (csrc/feature_slic.cuh): superpixels of float32 [B,C,H,W] tensors -- RGB-D,
+"""SLIC over float feature maps on the GPU (csrc/float_slic.cuh): superpixels of float32 [B,C,H,W] tensors -- RGB-D,
 multispectral bands, float Lab, a network's feature maps -- with any number of channels::
 
     x = torch.cat([lab_float, depth[:, None] * alpha], 1)          # [B,4,H,W] float32 on the GPU
@@ -14,22 +14,21 @@ every argument is checked (ValueError) before any device work.  Not differentiab
 import collections
 import ctypes
 import math
-import operator
 
 import torch
 
 from . import _lib
-from ._labelmaps import MAX_K, MAX_PIXELS, check_int, chunk, tensor
+from ._labelmaps import FLOAT_SLIC_MAX_C as MAX_C
+from ._labelmaps import FLOAT_SLIC_MAX_NODES as MAX_NODES
+from ._labelmaps import FLOAT_SLIC_MAX_SIDE as MAX_SIDE
+from ._labelmaps import FLOAT_SLIC_MAX_STRIDE as MAX_STRIDE
+from ._labelmaps import MAX_K, MAX_PIXELS, check_int, check_number, chunk, slic_dispatch, slic_pass_tiles, tensor
 from .base_slic import _locked, get_cca_engine
 
-MAX_C = 1024
-MAX_SIDE = 32767
-MAX_NODES = 1 << 30
-MAX_STRIDE = 255
 # Device memory one launch takes for its scratch at most (about 16 bytes per pass-row pixel, plus 4 * C + 8 per
 # cluster): a batch that needs more runs in chunks of images, with identical results.
 FEATURE_SLIC_SCRATCH_CAP = 1 << 30
-TILE_W, TILE_R = 32, 8  # FS_TILE_W, FS_TILE_R of feature_slic.cuh
+TILE_W, TILE_R = 32, 8  # MapSlic::TILE_W, TILE_R of float_slic.cuh
 
 FeatureSlic = collections.namedtuple("FeatureSlic", "labels position features count")
 FeatureSlic.__doc__ = """labels int16 [B,H,W] after connectivity enforcement; position float32 [B,K,2] (y, x),
@@ -49,12 +48,6 @@ def min_size_threshold(S, min_size_factor):
     return int(t + 1 if x - t >= 0.5 else t)
 
 
-def _number(name, v):
-    if isinstance(v, bool) or not isinstance(v, (int, float)) and not hasattr(v, "__float__"):
-        raise ValueError("%s must be a number, got %r" % (name, v))
-    return float(v)
-
-
 def _check(features, K, compactness, max_iter, subsample_stride, min_size_factor, init):
     tensor("features", features, torch.float32, 4)
     B, C, H, W = (int(v) for v in features.shape)
@@ -66,12 +59,12 @@ def _check(features, K, compactness, max_iter, subsample_stride, min_size_factor
     K = check_int("K", K, 1, min(MAX_K, H * W))
     if B * K > MAX_NODES:
         raise ValueError("B*K must be at most %d, got %d" % (MAX_NODES, B * K))
-    compactness = _number("compactness", compactness)
+    compactness = check_number("compactness", compactness)
     if not (math.isfinite(compactness) and compactness > 0) or not math.isfinite(ctypes.c_float(compactness).value):
         raise ValueError("compactness must be finite and > 0, got %r" % compactness)
     max_iter = check_int("max_iter", max_iter, 0, 2 ** 31 - 2)
     subsample_stride = check_int("subsample_stride", subsample_stride, 1, MAX_STRIDE)
-    min_size_factor = _number("min_size_factor", min_size_factor)
+    min_size_factor = check_number("min_size_factor", min_size_factor)
     if not min_size_factor >= 0:
         raise ValueError("min_size_factor must be >= 0, got %r" % min_size_factor)
     if init is not None:
@@ -142,22 +135,13 @@ def feature_slic(features, K, compactness, max_iter=10, subsample_stride=3, min_
 
 def pass_tiles(H, W, max_iter, subsample_stride):
     """Tiles per image of every assign pass: max_iter strided passes, then the full one."""
-    out = []
-    for t in range(max_iter + 1):
-        r, s = (t % subsample_stride, subsample_stride) if t < max_iter else (0, 1)
-        npr = (H - 1 - r) // s + 1 if r < H else 0
-        out.append(-(-W // TILE_W) * -(-npr // TILE_R))
-    return out
+    return slic_pass_tiles((H, W), (TILE_R, TILE_W), max_iter, subsample_stride)
 
 
 def feature_slic_dispatch(features, K, compactness, max_iter=10, subsample_stride=3, min_size_factor=0.25, init=None):
     """feature_slic with a record of the assign kernels it ran (synchronises): (result, [(tiles, overflowed)] per
     pass), the tiles of the pass over the whole batch and how many of them overflowed the tile kernel's candidate
     list and went to the per-pixel kernel."""
-    B = int(features.shape[0]) if isinstance(features, torch.Tensor) else 0
-    max_iter = operator.index(max_iter)
-    overflow = torch.zeros((max(B, 1), max_iter + 1), dtype=torch.int32, device=features.device)
-    r = _run(features, K, compactness, max_iter, subsample_stride, min_size_factor, init, overflow)
-    H, W = int(features.shape[2]), int(features.shape[3])
-    tiles = pass_tiles(H, W, max_iter, subsample_stride)
-    return r, [(B * t, int(o)) for t, o in zip(tiles, overflow.sum(0).tolist())]
+    return slic_dispatch(lambda it, overflow: _run(features, K, compactness, it, subsample_stride, min_size_factor,
+                                                   init, overflow), features, max_iter, subsample_stride,
+                         (TILE_R, TILE_W))

@@ -23,9 +23,9 @@ import torch
 from torch.autograd.function import once_differentiable
 
 from . import _lib
-from ._labelmaps import MAX_K, MAX_PIXELS, check_int, tensor
+from ._labelmaps import MAX_K, MAX_PIXELS, check_int, check_number, tensor
 from .base_slic import _locked, get_cca_engine
-from .feature_slic import _number, min_size_threshold, superpixel_size
+from .feature_slic import min_size_threshold, superpixel_size
 from .pooling import pool
 
 MAX_NODES = 1 << 30
@@ -281,7 +281,7 @@ def soft_slic(features, num_cells, n_iter=5, min_size_factor=0.25):
     _nodes(B, K)
     n_iter = check_int("n_iter", n_iter, 1, 2 ** 31 - 1)
     if min_size_factor is not None:
-        min_size_factor = _number("min_size_factor", min_size_factor)
+        min_size_factor = check_number("min_size_factor", min_size_factor)
         if not min_size_factor >= 0:
             raise ValueError("min_size_factor must be >= 0 or None, got %r" % min_size_factor)
     dev = _device(("features", features))

@@ -1,4 +1,4 @@
-"""Supervoxels on the GPU (csrc/supervoxel.cuh, csrc/sv_cca.cuh): SLIC over float32 volumes [B,C,D,H,W] -- CT, MRI,
+"""Supervoxels on the GPU (csrc/float_slic.cuh, csrc/sv_cca.cuh): SLIC over float32 volumes [B,C,D,H,W] -- CT, MRI,
 microscopy stacks -- with a voxel spacing, and connectivity enforcement of label volumes in 6-connectivity::
 
     x = ct[:, None]                                                                        # [B,1,D,H,W] float32
@@ -14,22 +14,20 @@ graph can capture it; every argument is checked (ValueError) before any device w
 """
 import collections
 import math
-import operator
 
 import numpy as np
 import torch
 
 from . import _lib
-from ._labelmaps import MAX_K, MAX_PIXELS, check_int, chunk, tensor
-
-MAX_C = 1024
-MAX_SIDE = 32767
-MAX_NODES = 1 << 30
-MAX_STRIDE = 255
+from ._labelmaps import FLOAT_SLIC_MAX_C as MAX_C
+from ._labelmaps import FLOAT_SLIC_MAX_NODES as MAX_NODES
+from ._labelmaps import FLOAT_SLIC_MAX_SIDE as MAX_SIDE
+from ._labelmaps import FLOAT_SLIC_MAX_STRIDE as MAX_STRIDE
+from ._labelmaps import MAX_K, MAX_PIXELS, check_int, check_number, chunk, slic_dispatch, slic_pass_tiles, tensor
 # Device memory one launch takes for its scratch at most (about 20 bytes per voxel for the enforcement, more for the
 # passes at large C): a batch that needs more runs in chunks of volumes, with identical results.
 SUPERVOXEL_SCRATCH_CAP = 1 << 30
-TILE_W, TILE_R, TILE_D = 16, 4, 4  # SV_TILE_W, SV_TILE_R, SV_TILE_D of supervoxel.cuh
+TILE_W, TILE_R, TILE_D = 16, 4, 4  # VolumeSlic::TILE_W, TILE_R, TILE_D of float_slic.cuh
 
 Supervoxels = collections.namedtuple("Supervoxels", "labels position features count grid")
 Supervoxels.__doc__ = """labels int16 [B,D,H,W] after connectivity enforcement (read them as uint16 when K' > 32767);
@@ -38,16 +36,10 @@ update (the seeds when max_iter == 0, count 0 then), which describe the labels b
 K' = nd * nh * nw."""
 
 
-def _number(name, v):
-    if isinstance(v, bool) or not isinstance(v, (int, float)) and not hasattr(v, "__float__"):
-        raise ValueError("%s must be a number, got %r" % (name, v))
-    return float(v)
-
-
 def _spacing(spacing):
     if not isinstance(spacing, (tuple, list)) or len(spacing) != 3:
         raise ValueError("spacing must be (z, y, x), got %r" % (spacing,))
-    sp = tuple(_number("spacing", v) for v in spacing)
+    sp = tuple(check_number("spacing", v) for v in spacing)
     if not all(math.isfinite(v) and v > 0 for v in sp):
         raise ValueError("spacing must be finite and > 0, got %r" % (spacing,))
     return sp
@@ -110,7 +102,7 @@ def _check(volumes, K, compactness, spacing, max_iter, subsample_stride, min_siz
     Kp = grid[0] * grid[1] * grid[2]
     if B * Kp > MAX_NODES:
         raise ValueError("B*K' must be at most %d, got %d" % (MAX_NODES, B * Kp))
-    compactness = _number("compactness", compactness)
+    compactness = check_number("compactness", compactness)
     if not (math.isfinite(compactness) and compactness > 0):
         raise ValueError("compactness must be finite and > 0, got %r" % compactness)
     w2 = weights(D, H, W, grid, compactness, sp)
@@ -118,7 +110,7 @@ def _check(volumes, K, compactness, spacing, max_iter, subsample_stride, min_siz
         raise ValueError("compactness * spacing / s overflows float32 when squared: %r" % (w2,))
     max_iter = check_int("max_iter", max_iter, 0, 2 ** 31 - 2)
     subsample_stride = check_int("subsample_stride", subsample_stride, 1, MAX_STRIDE)
-    min_size_factor = _number("min_size_factor", min_size_factor)
+    min_size_factor = check_number("min_size_factor", min_size_factor)
     if not (math.isfinite(min_size_factor) and min_size_factor >= 0):
         raise ValueError("min_size_factor must be finite and >= 0, got %r" % min_size_factor)
     if volumes.device.type != "cuda":
@@ -213,12 +205,7 @@ def enforce_connectivity_3d(labels, K, min_size):
 
 def pass_tiles(D, H, W, max_iter, subsample_stride):
     """Tiles per volume of every assign pass: max_iter strided passes, then the full one."""
-    out = []
-    for t in range(max_iter + 1):
-        r, s = (t % subsample_stride, subsample_stride) if t < max_iter else (0, 1)
-        npr = (H - 1 - r) // s + 1 if r < H else 0
-        out.append(-(-W // TILE_W) * -(-npr // TILE_R) * -(-D // TILE_D))
-    return out
+    return slic_pass_tiles((D, H, W), (TILE_D, TILE_R, TILE_W), max_iter, subsample_stride)
 
 
 def supervoxel_dispatch(volumes, K, compactness, spacing=(1.0, 1.0, 1.0), max_iter=10, subsample_stride=3,
@@ -226,10 +213,6 @@ def supervoxel_dispatch(volumes, K, compactness, spacing=(1.0, 1.0, 1.0), max_it
     """supervoxel_slic with a record of the assign kernels it ran (synchronises): (result, [(tiles, overflowed)] per
     pass), the tiles of the pass over the whole batch and how many of them overflowed the tile kernel's candidate list
     and went to the per-voxel kernel."""
-    B = int(volumes.shape[0]) if isinstance(volumes, torch.Tensor) else 0
-    max_iter = operator.index(max_iter)
-    overflow = torch.zeros((max(B, 1), max_iter + 1), dtype=torch.int32, device=volumes.device)
-    r = _run(volumes, K, compactness, spacing, max_iter, subsample_stride, min_size_factor, overflow)
-    D, H, W = (int(v) for v in volumes.shape[2:])
-    tiles = pass_tiles(D, H, W, max_iter, subsample_stride)
-    return r, [(B * t, int(o)) for t, o in zip(tiles, overflow.sum(0).tolist())]
+    return slic_dispatch(lambda it, overflow: _run(volumes, K, compactness, spacing, it, subsample_stride,
+                                                   min_size_factor, overflow), volumes, max_iter, subsample_stride,
+                         (TILE_D, TILE_R, TILE_W))

@@ -97,7 +97,7 @@ def main():
         run = lambda: feature_slic(x, K, a.compactness, a.max_iter, a.stride)  # noqa: E731
         med, lo, hi = timed(run, a.reps, a.warmup)
         kt = kernel_times(run)
-        tiles = kt.get("k_fs_assign_tiles", [])
+        tiles = kt.get("k_float_slic_assign_tiles", [])
         # the passes' visited pixels: max_iter strided passes, then the full one
         visited = [B * len(range(t % a.stride, H, a.stride)) * W for t in range(a.max_iter)] + [B * H * W]
         assign_bytes = [v * (4 * C + 2) for v in visited]

@@ -117,8 +117,8 @@ def main():
         kt = kernel_times(run)
         total = sum(sum(v) for v in kt.values())
         enforce = sum(sum(v) for k, v in kt.items() if k.startswith("k_svc"))
-        tiles = kt.get("k_sv_assign_tiles", [])
-        fallback = kt.get("k_sv_assign_fallback", [])
+        tiles = kt.get("k_float_slic_assign_tiles", [])
+        fallback = kt.get("k_float_slic_assign_fallback", [])
         n = B * D * H * W
         full_bytes = n * (4 * C + 2)
         chunks = len(tiles) // (a.max_iter + 1) if tiles else 0
