@@ -55,6 +55,16 @@ def check_connectivity(connectivity):
     return connectivity
 
 
+def check_connectivity_3d(connectivity):
+    try:
+        connectivity = operator.index(connectivity)
+    except TypeError:
+        raise ValueError("connectivity must be 6, 18 or 26, got %r" % (connectivity,)) from None
+    if connectivity not in (6, 18, 26):
+        raise ValueError("connectivity must be 6, 18 or 26, got %r" % (connectivity,))
+    return connectivity
+
+
 def check_pixels(H, W, reason=""):
     """Images of at most MAX_PIXELS pixels; `reason` ends the message."""
     if H * W > MAX_PIXELS:

@@ -40,10 +40,11 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_pool_batch_scratch_bytes", "fslic_b200_pool_batch", "fslic_b200_pool_unpool_batch",
     "fslic_b200_pool_paint_argmax_batch", "fslic_b200_pool_paint_batch",
     "fslic_b200_rag_batch_scratch_bytes", "fslic_b200_rag_batch_count", "fslic_b200_rag_fill_scratch_bytes",
-    "fslic_b200_rag_batch_fill",
+    "fslic_b200_rag_batch_fill", "fslic_b200_rag3d_batch_scratch_bytes", "fslic_b200_rag3d_batch_count",
+    "fslic_b200_rag3d_batch_fill",
     "fslic_b200_gt_histogram_batch", "fslic_b200_gt_scores_scratch_bytes", "fslic_b200_gt_scores_batch",
     "fslic_b200_gt_boundaries_batch",
-    "fslic_b200_props_batch",
+    "fslic_b200_props_batch", "fslic_b200_props3d_batch",
     "fslic_b200_merge_scratch_bytes", "fslic_b200_merge_batch",
     "fslic_b200_boundary_select_scratch_bytes", "fslic_b200_boundary_select_batch",
     "fslic_b200_boundary_stats_scratch_bytes", "fslic_b200_boundary_stats_batch",
@@ -149,6 +150,10 @@ def lib():
     L.fslic_b200_rag_fill_scratch_bytes.restype = C.c_size_t
     L.fslic_b200_rag_batch_fill.argtypes = [i32, i32, i32, i32, i32, i32, i32, i64, i64, vp, C.c_size_t, vp, C.c_size_t,
                                             vp, vp, vp, vp]
+    L.fslic_b200_rag3d_batch_scratch_bytes.argtypes = [i32] * 7
+    L.fslic_b200_rag3d_batch_scratch_bytes.restype = C.c_size_t
+    L.fslic_b200_rag3d_batch_count.argtypes = [i32] * 8 + [vp, i64, vp, vp, vp, C.c_size_t, vp]
+    L.fslic_b200_rag3d_batch_fill.argtypes = [i32] * 8 + [i64, i64, vp, C.c_size_t, vp, C.c_size_t, vp, vp, vp, vp]
     L.fslic_b200_gt_histogram_batch.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp]
     L.fslic_b200_gt_scores_scratch_bytes.argtypes = [i32, i32, i32, i32]
     L.fslic_b200_gt_scores_scratch_bytes.restype = C.c_size_t
@@ -156,6 +161,7 @@ def lib():
                                              vp]
     L.fslic_b200_gt_boundaries_batch.argtypes = [i32, i32, i32, i32, vp, vp, vp]
     L.fslic_b200_props_batch.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.fslic_b200_props3d_batch.argtypes = [i32] * 6 + [vp] * 9
     L.fslic_b200_merge_scratch_bytes.argtypes = [i32, i32]
     L.fslic_b200_merge_scratch_bytes.restype = C.c_size_t
     L.fslic_b200_merge_batch.argtypes = [i32, i32, i32, i32, i32, vp, i64, vp, vp, vp, i32, C.c_double, i32, vp, vp, vp,

@@ -8,6 +8,8 @@
 //                   plus down-right and down-left.  Lanes of a warp holding the same (image, key) add once (MATCH.ANY);
 //                   the leader claims a slot with one CAS and adds the count with one atomicAdd.  Past max_probes the
 //                   image's overflow flag is set;
+//   k_rag3d_discover the same over volumes (section 4.23): one thread per voxel, 3, 9 or 13 voxel pairs each
+//                   (connectivity 6, 18, 26), feeding the same tables; every later step is shared;
 //   k_rag_degree    every occupied slot adds 1 to the degree of both of its labels;
 //   (exclusive scan of the degrees: the call-local CSR row offsets)
 //   k_rag_finish    the caller's row offsets (shifted by the edges of earlier calls) and the call's edge total;
@@ -68,6 +70,89 @@ __global__ void __launch_bounds__(256) k_rag_discover(const uint16_t* __restrict
                 }
                 h = (h + 1) & tmask;
             }
+        }
+    }
+}
+
+// k_rag_discover's insert of one direction as a function for k_rag3d_discover (the 2-D kernel keeps its own copy, so
+// its code is unchanged), called by all 32 lanes: lanes holding the same (image, key) add once (MATCH.ANY), the leader
+// claims a slot of image b's table with one CAS and adds the lane count; past max_probes the image's flag is set.  A
+// key of ~0 is no pair.
+__device__ __forceinline__ void rag_add(unsigned long long key, int lane, long b, uint32_t* __restrict__ tkey,
+                                        uint32_t* __restrict__ tcnt, uint32_t T, uint32_t max_probes,
+                                        long long* __restrict__ overflow) {
+    const unsigned peers = __match_any_sync(FSLIC_FULL, key);
+    if (key == ~0ull || lane != __ffs(peers) - 1) return;
+    const uint32_t k32 = (uint32_t)key;
+    const uint32_t tmask = T - 1;
+    uint32_t* ks = tkey + b * T;
+    uint32_t h = conn_hash(k32) & tmask;
+    for (uint32_t probes = 0;; probes++) {
+        if (probes >= max_probes) {
+            overflow[b] = 1;
+            break;
+        }
+        const uint32_t old = atomicCAS(&ks[h], RAG_EMPTY, k32);
+        if (old == RAG_EMPTY || old == k32) {
+            atomicAdd(&tcnt[b * T + h], (uint32_t)__popc(peers));
+            break;
+        }
+        h = (h + 1) & tmask;
+    }
+}
+
+// k_rag_discover over volumes: one thread per voxel, 3 (connectivity 6), 9 (18) or 13 (26) voxel pairs each.  Every
+// direction is tested first and one warp vote skips warps whose voxels all lie inside one label (most of a supervoxel
+// map); the rest go through the same per-direction vote, match and table insert as the 2-D kernel.
+template <int CONN>
+__global__ void __launch_bounds__(256) k_rag3d_discover(const uint16_t* __restrict__ lab, long dhw, int D, int H, int W,
+                                                         long n, int K, uint32_t* __restrict__ tkey,
+                                                         uint32_t* __restrict__ tcnt, uint32_t T, uint32_t max_probes,
+                                                         long long* __restrict__ overflow) {
+    // the forward half of the 3x3x3 neighbourhood (first non-zero offset positive), (dz, dy, dx): connectivity 6 takes
+    // the first 3 (faces), 18 the first 9 (and edges), 26 all 13 (and corners)
+    constexpr int NDIR = CONN == 6 ? 3 : (CONN == 18 ? 9 : 13);
+    constexpr int8_t dirs[13][3] = {{0, 0, 1}, {0, 1, 0},  {1, 0, 0},  {0, 1, 1},  {0, 1, -1},
+                                    {1, 1, 0}, {1, -1, 0}, {1, 0, 1},  {1, 0, -1}, {1, 1, 1},
+                                    {1, 1, -1}, {1, -1, 1}, {1, -1, -1}};
+    const long step = (long)gridDim.x * blockDim.x;
+    const long nround = (n + step - 1) / step * step;  // whole warps stay in the loop: the warp intrinsics need all lanes
+    const int lane = threadIdx.x & 31;
+    const uint32_t hw = (uint32_t)H * (uint32_t)W;
+    for (long t = (long)blockIdx.x * blockDim.x + threadIdx.x; t < nround; t += step) {
+        long b = 0;
+        int z = 0, y = 0, x = 0;
+        uint32_t s = 0xffffu;
+        if (t < n) {
+            // 32-bit divisions where they suffice (dhw <= 2^29), a 64-bit one only for calls of 2^32 voxels or more
+            b = n <= (long)UINT32_MAX ? (long)((uint32_t)t / (uint32_t)dhw) : t / dhw;
+            const uint32_t p = (uint32_t)(t - b * dhw);
+            z = (int)(p / hw);
+            const uint32_t r = p - (uint32_t)z * hw;
+            y = (int)(r / (uint32_t)W);
+            x = (int)(r - (uint32_t)y * (uint32_t)W);
+            s = lab[t];
+        }
+        // bit d: the pair in direction d is valid and its labels differ
+        uint32_t diff = 0;
+#pragma unroll
+        for (int d = 0; d < NDIR; d++) {
+            const int dz = dirs[d][0], dy = dirs[d][1], dx = dirs[d][2];
+            if (s < (uint32_t)K && z + dz < D && y + dy >= 0 && y + dy < H && x + dx >= 0 && x + dx < W) {
+                const uint32_t g = lab[t + (long)dz * hw + (long)dy * W + dx];
+                if (g < (uint32_t)K && g != s) diff |= 1u << d;
+            }
+        }
+        if (!__any_sync(FSLIC_FULL, diff != 0)) continue;  // most warps: no boundary in any direction
+#pragma unroll
+        for (int d = 0; d < NDIR; d++) {
+            if (!__any_sync(FSLIC_FULL, diff >> d & 1u)) continue;
+            unsigned long long key = ~0ull;
+            if (diff >> d & 1u) {  // the neighbour again, from L1
+                const uint32_t g = lab[t + (long)dirs[d][0] * hw + (long)dirs[d][1] * W + dirs[d][2]];
+                key = (unsigned long long)b << 32 | (s < g ? s << 16 | g : g << 16 | s);
+            }
+            rag_add(key, lane, b, tkey, tcnt, T, max_probes, overflow);
         }
     }
 }

@@ -21,7 +21,8 @@ by the lower index, in the same node numbering and CSR layout::
 
 No counterpart in the reference: its get_connectivity keeps at most 12 neighbours per superpixel, in scan order, and
 is kept for parity with it; its get_knn_connectivity has no defined result and raises NotImplementedError here.
-DESIGN.md sections 4.13, 4.17 and 4.18 describe the kernels.
+region_adjacency_3d is the graph of supervoxel label volumes [B,D,H,W], in 6-, 18- or 26-connectivity.  DESIGN.md
+sections 4.13, 4.17, 4.18 and 4.23 describe the kernels.
 """
 import collections
 
@@ -29,8 +30,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._labelmaps import (MAX_PIXELS, NO_SIZE, check_connectivity, check_features, check_graph, check_int, check_K,
-                         check_pixels, chunk, cuda_device, tensor)
+from ._labelmaps import (MAX_PIXELS, NO_SIZE, check_connectivity, check_connectivity_3d, check_features, check_graph,
+                         check_int, check_K, check_pixels, chunk, cuda_device, tensor)
 
 # Device memory the pair tables of one count launch take at most (8 bytes per slot, a power of two >= max(4096, 32 K)
 # slots per image): a batch that needs more runs in chunks of images, with identical results.
@@ -47,6 +48,11 @@ _INT_MAX = 2 ** 31 - 1
 KNN_MAX_D = 64
 KNN_MAX_NEIGHBORS = 32
 KNN_MAX_NODES = 1 << 30  # B * K
+
+# The forward half of the 3x3x3 neighbourhood, (dz, dy, dx) with the first non-zero component positive: the voxel
+# pairs of region_adjacency_3d are each voxel with these neighbours (connectivity 6: the first 3, 18: 9, 26: 13)
+RAG3D_OFFSETS = ((0, 0, 1), (0, 1, 0), (1, 0, 0), (0, 1, 1), (0, 1, -1), (1, 1, 0), (1, -1, 0), (1, 0, 1), (1, 0, -1),
+                 (1, 1, 1), (1, 1, -1), (1, -1, 1), (1, -1, -1))
 
 RegionGraph = collections.namedtuple("RegionGraph", ["indptr", "edge_index", "boundary"])
 BoundaryStats = collections.namedtuple("BoundaryStats", ["mean", "min", "max", "count"])
@@ -109,50 +115,116 @@ def region_adjacency(labels, K, connectivity=4):
             return RegionGraph(torch.zeros(B * K + 1, dtype=torch.int64, device=dev),
                                torch.empty((2, 0), dtype=torch.int64, device=dev),
                                torch.empty(0, dtype=torch.int32, device=dev))
-        lab = labels.contiguous()
         L = _lib.lib()
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        indptr = torch.empty(B * K + 1, dtype=torch.int64, device=dev)
-        chunk = rag_chunk(B, H, W, K, connectivity)
-        work = [(b0, min(chunk, B - b0), 0) for b0 in range(0, B, chunk)][::-1]
-        pieces, edges = [], 0
-        while work:
-            b0, c, exact = work.pop()
-            nbytes = int(L.fslic_b200_rag_batch_scratch_bytes(c, H, W, K, connectivity, exact))
-            if nbytes == NO_SIZE:
-                raise MemoryError("image %d has too many distinct adjacent label pairs for an exact pair table" % b0)
-            scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            info = torch.empty(c + 1, dtype=torch.int64, device=dev)
-            _lib.check(L.fslic_b200_rag_batch_count(dev.index, c, H, W, K, connectivity, exact, lab[b0].data_ptr(), edges,
-                                                    indptr[b0 * K:].data_ptr(), info.data_ptr(), scratch.data_ptr(),
-                                                    nbytes, stream))
-            info = info.tolist()  # the host wait: overflow flags and the edge total
-            flags, total = info[:c], info[c]
-            if any(flags):
-                work.extend(_split(b0, flags)[::-1])
-                continue
-            if total > _INT_MAX:  # one segmented sort per fill
-                if c == 1:
-                    raise MemoryError("image %d has %d directed edges, more than one fill takes" % (b0, total))
-                work.extend([(b0 + c // 2, c - c // 2, exact), (b0, c // 2, exact)])
-                continue
-            edge_index = torch.empty((2, total), dtype=torch.int64, device=dev)
-            boundary = torch.empty(total, dtype=torch.int32, device=dev)
-            if total:
-                fbytes = int(L.fslic_b200_rag_fill_scratch_bytes(c, K, total))
-                fill = torch.empty(fbytes, dtype=torch.uint8, device=dev)
-                _lib.check(L.fslic_b200_rag_batch_fill(dev.index, c, H, W, K, connectivity, exact, b0 * K, total,
-                                                       scratch.data_ptr(), nbytes, fill.data_ptr(), fbytes,
-                                                       edge_index[0].data_ptr(), edge_index[1].data_ptr(),
-                                                       boundary.data_ptr(), stream))
-            pieces.append((edge_index, boundary))
-            edges += total
-        if len(pieces) == 1:
-            edge_index, boundary = pieces[0]
-        else:
-            edge_index = torch.cat([p[0] for p in pieces], dim=1)
-            boundary = torch.cat([p[1] for p in pieces])
+        return _rag(labels.contiguous(), B, K, rag_chunk(B, H, W, K, connectivity), (H, W, K, connectivity), "image",
+                    L.fslic_b200_rag_batch_scratch_bytes, L.fslic_b200_rag_batch_count, L.fslic_b200_rag_batch_fill)
+
+
+def _rag(lab, B, K, first_chunk, dims, what, scratch_bytes, count, fill):
+    """The count / read / fill loop of region_adjacency and region_adjacency_3d over B contiguous images or volumes
+    lab on the current device: chunks of first_chunk, overflowed ones split by _split and recounted, those of more
+    than 2^31 - 1 edges halved.  dims are the entry points' arguments between the batch and `exact`."""
+    dev = lab.device
+    L = _lib.lib()
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    indptr = torch.empty(B * K + 1, dtype=torch.int64, device=dev)
+    work = [(b0, min(first_chunk, B - b0), 0) for b0 in range(0, B, first_chunk)][::-1]
+    pieces, edges = [], 0
+    while work:
+        b0, c, exact = work.pop()
+        nbytes = int(scratch_bytes(c, *dims, exact))
+        if nbytes == NO_SIZE:
+            raise MemoryError("%s %d has too many distinct adjacent label pairs for an exact pair table" % (what, b0))
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        info = torch.empty(c + 1, dtype=torch.int64, device=dev)
+        _lib.check(count(dev.index, c, *dims, exact, lab[b0].data_ptr(), edges, indptr[b0 * K:].data_ptr(),
+                         info.data_ptr(), scratch.data_ptr(), nbytes, stream))
+        info = info.tolist()  # the host wait: overflow flags and the edge total
+        flags, total = info[:c], info[c]
+        if any(flags):
+            work.extend(_split(b0, flags)[::-1])
+            continue
+        if total > _INT_MAX:  # one segmented sort per fill
+            if c == 1:
+                raise MemoryError("%s %d has %d directed edges, more than one fill takes" % (what, b0, total))
+            work.extend([(b0 + c // 2, c - c // 2, exact), (b0, c // 2, exact)])
+            continue
+        edge_index = torch.empty((2, total), dtype=torch.int64, device=dev)
+        boundary = torch.empty(total, dtype=torch.int32, device=dev)
+        if total:
+            fbytes = int(L.fslic_b200_rag_fill_scratch_bytes(c, K, total))
+            fill_scratch = torch.empty(fbytes, dtype=torch.uint8, device=dev)
+            _lib.check(fill(dev.index, c, *dims, exact, b0 * K, total, scratch.data_ptr(), nbytes,
+                            fill_scratch.data_ptr(), fbytes, edge_index[0].data_ptr(), edge_index[1].data_ptr(),
+                            boundary.data_ptr(), stream))
+        pieces.append((edge_index, boundary))
+        edges += total
+    if len(pieces) == 1:
+        edge_index, boundary = pieces[0]
+    else:
+        edge_index = torch.cat([p[0] for p in pieces], dim=1)
+        boundary = torch.cat([p[1] for p in pieces])
     return RegionGraph(indptr, edge_index, boundary)
+
+
+def voxel_pairs(D, H, W, connectivity):
+    """Voxel pairs of one D x H x W volume at connectivity 6, 18 or 26: sum over the forward offsets (dz, dy, dx) with
+    at most 1, 2 or 3 non-zero components of (D - |dz|)(H - |dy|)(W - |dx|)."""
+    if D * H * W == 0:
+        return 0
+    most = {6: 1, 18: 2, 26: 3}[connectivity]
+    return sum((D - abs(dz)) * (H - abs(dy)) * (W - abs(dx)) for dz, dy, dx in RAG3D_OFFSETS
+               if (dz != 0) + (dy != 0) + (dx != 0) <= most)
+
+
+def rag3d_chunk(B, D, H, W, K, connectivity):
+    """Volumes per count launch of region_adjacency_3d: as many as fit RAG_SCRATCH_CAP, at least one."""
+    f = _lib.lib().fslic_b200_rag3d_batch_scratch_bytes
+    if f(1, D, H, W, K, connectivity, 0) == NO_SIZE:
+        raise ValueError("a volume of %dx%dx%d voxels is too large for a region adjacency graph" % (D, H, W))
+    return chunk(lambda c: f(c, D, H, W, K, connectivity, 0), RAG_SCRATCH_CAP, B)
+
+
+def region_adjacency_3d(labels, K, connectivity=6):
+    """Region adjacency graph of int16 label volumes [B,D,H,W] (read as uint16) -> RegionGraph(indptr, edge_index,
+    boundary), the volume form of region_adjacency with the same node numbering n = b*K + k, dtypes and CSR / COO
+    layout, so every consumer of region_adjacency's graph (merge_regions, knn_graph's users, message_passing) takes it.
+    - boundary int32 [E]: the number of adjacent voxel pairs whose labels are the edge's two nodes.
+    Voxel pairs are the forward half of the 3x3x3 neighbourhood, each unordered pair once, the last slice, row and
+    column included: the 3 face neighbours (connectivity=6), plus the 6 edge neighbours (18), plus the 4 corner
+    neighbours (26).  A label outside [0, K) (-1 included) belongs to no node and its pairs are ignored; a pair with
+    equal labels is no edge.  1 <= K <= 65534, D * H * W <= 2^29 and the volume's voxel pair count (voxel_pairs) at
+    most 2^31 - 1 (so every boundary count fits int32: a 512^3 volume fits at 26-connectivity; 2^29 voxels at 18 or
+    26 do not); anything else, a tensor that is not a cuda int16 [B,D,H,W] tensor, or a connectivity other than 6, 18
+    or 26 raises ValueError before any device work.  B, D, H or W = 0 gives zero rows and no edges.
+
+    Host behaviour is region_adjacency's: one read of (volumes + 1) int64 words per chunk of volumes
+    (RAG_SCRATCH_CAP), volumes whose pair table overflowed counted again alone with an exact table, RuntimeError under
+    CUDA graph capture before any device work.  All arithmetic is integer: the result is exact and the same across
+    runs, batch order, chunking and streams."""
+    tensor("labels", labels, torch.int16, 4)
+    connectivity = check_connectivity_3d(connectivity)
+    K = check_K(K)
+    B, D, H, W = (int(v) for v in labels.shape)
+    if D * H * W > MAX_PIXELS:
+        raise ValueError("volumes of %dx%dx%d voxels exceed %d voxels" % (D, H, W, MAX_PIXELS))
+    P = voxel_pairs(D, H, W, connectivity)
+    if P > _INT_MAX:
+        raise ValueError("volumes of %dx%dx%d voxels have %d voxel pairs at connectivity %d, more than %d: a "
+                         "boundary count could overflow int32" % (D, H, W, P, connectivity, _INT_MAX))
+    dev = cuda_device(labels)
+    with torch.cuda.device(dev):
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("region_adjacency_3d reads its edge count back to the host and cannot be captured in a "
+                               "CUDA graph")
+        if B == 0 or D == 0 or H == 0 or W == 0:
+            return RegionGraph(torch.zeros(B * K + 1, dtype=torch.int64, device=dev),
+                               torch.empty((2, 0), dtype=torch.int64, device=dev),
+                               torch.empty(0, dtype=torch.int32, device=dev))
+        L = _lib.lib()
+        return _rag(labels.contiguous(), B, K, rag3d_chunk(B, D, H, W, K, connectivity), (D, H, W, K, connectivity),
+                    "volume", L.fslic_b200_rag3d_batch_scratch_bytes, L.fslic_b200_rag3d_batch_count,
+                    L.fslic_b200_rag3d_batch_fill)
 
 
 def boundary_chunk(B, H, W, K, connectivity):

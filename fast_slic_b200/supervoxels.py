@@ -160,8 +160,10 @@ def supervoxel_slic(volumes, K, compactness, spacing=(1.0, 1.0, 1.0), max_iter=1
     members to their mean position and pooled mean features; one assign over every voxel follows, then
     enforce_connectivity_3d with min_size = round(min_size_factor * D*H*W / K').  compactness has no default: the
     feature distance has no fixed scale.  At D = 1 this is not feature_slic: the seed grids and windows differ.
-    Per-supervoxel statistics come from pooling.pool over the volume viewed as [B,C,D*H,W]; region_adjacency,
-    region_properties and the boundary metrics are 2-D and give wrong answers on a reshaped volume.  Limits:
+    Per-supervoxel statistics come from pooling.pool over the volume viewed as [B,C,D*H,W]; the supervoxel graph from
+    region_graph.region_adjacency_3d and the shapes from geometry.region_properties_3d.  merge_regions, pool,
+    class_histogram and the ASA / undersegmentation fields of segmentation_scores read labels per voxel and are correct
+    on the [B,D*H,W] view; boundaries and the boundary-recall fields of segmentation_scores remain 2-D.  Limits:
     1 <= C <= 1024, D, H, W <= 32767, D*H*W <= 2^29, K' <= 65534, B*K' <= 2^30, 1 <= subsample_stride <= 255, spacing
     finite and > 0."""
     return _run(volumes, K, compactness, spacing, max_iter, subsample_stride, min_size_factor)

@@ -270,6 +270,22 @@ int fslic_b200_rag_batch_fill(int device, int batch, int H, int W, int K, int co
                               long long node_base, long long edges, const void* d_scratch, size_t scratch_bytes,
                               void* d_fill_scratch, size_t fill_bytes, long long* d_src, long long* d_dst,
                               int32_t* d_boundary, void* stream);
+/* Region adjacency graphs of `batch` label volumes d_labels u16[B,D,H,W] (DESIGN.md section 4.23): the same graph,
+ * tables, calls and outputs as above, with voxel pairs for pixel pairs.  Voxel pairs are the forward half of the
+ * 3x3x3 neighbourhood (offsets (dz, dy, dx) whose first non-zero component is positive) with at most 1 (connectivity
+ * 6), 2 (18) or 3 (26) non-zero components: 3, 9 or 13 per voxel.  D * H * W <= 2^29, and the volume's pair count
+ * P = sum over those offsets of (D - |dz|)(H - |dy|)(W - |dx|) must be at most 2^31 - 1, so that every boundary count
+ * fits int32.  Scratch bytes as fslic_b200_rag_batch_scratch_bytes with P for the pixel pairs; (size_t)-1 for bad
+ * arguments, D * H * W > 2^29, P > 2^31 - 1, B * K >= 2^31 - 1 or an exact table over 2^31 slots.  The fill takes its
+ * scratch from fslic_b200_rag_fill_scratch_bytes. */
+size_t fslic_b200_rag3d_batch_scratch_bytes(int batch, int D, int H, int W, int K, int connectivity, int exact);
+int fslic_b200_rag3d_batch_count(int device, int batch, int D, int H, int W, int K, int connectivity, int exact,
+                                 const uint16_t* d_labels, long long edge_base, long long* d_indptr, long long* d_info,
+                                 void* d_scratch, size_t scratch_bytes, void* stream);
+int fslic_b200_rag3d_batch_fill(int device, int batch, int D, int H, int W, int K, int connectivity, int exact,
+                                long long node_base, long long edges, const void* d_scratch, size_t scratch_bytes,
+                                void* d_fill_scratch, size_t fill_bytes, long long* d_src, long long* d_dst,
+                                int32_t* d_boundary, void* stream);
 
 /* Superpixels scored against ground truth (groundtruth.cuh; no counterpart in the reference) over `batch` label maps
  * d_labels u16[B,H,W] and maps of the same shape whose element type is `dtype`, one of the FSLIC_GT_* codes (the element
@@ -317,6 +333,22 @@ int fslic_b200_gt_boundaries_batch(int device, int batch, int H, int W, const ui
 int fslic_b200_props_batch(int device, int batch, int H, int W, int K, const uint16_t* d_labels, int32_t* d_area,
                            int32_t* d_bbox, long long* d_moments, int32_t* d_perimeter, int32_t* d_border,
                            double* d_centroid, double* d_covariance, void* stream);
+/* Supervoxel shapes (props3d.cuh; DESIGN.md section 4.23) of `batch` label volumes d_labels u16[B,D,H,W]; node
+ * n = b*K + k, voxel (slice z, row y, column x) has coordinates (z, y, x).  A label outside [0, K) belongs to no
+ * supervoxel.  1 <= K <= 65534, D, H, W <= 32767, D * H * W <= 2^29.  Outputs, all device memory:
+ *   d_area int32[B*K]         voxels labelled k;
+ *   d_bbox int32[B*K][6]      (z0, y0, x0, z1, y1, x1): min inclusive, max exclusive; all 0 for an empty node;
+ *   d_moments int64[B*K][9]   (sum z, y, x, z^2, zy, zx, y^2, yx, x^2) over k's voxels, exact;
+ *   d_surface int64[B*K]      faces of k's voxels whose 6-neighbour across that face is outside the volume or has
+ *                             another raw label;
+ *   d_border int32[B*K]       those of the faces that lie on the volume's edge;
+ *   d_centroid f64[B*K][3]    (sum z / n, sum y / n, sum x / n);
+ *   d_covariance f64[B*K][6]  (zz, zy, zx, yy, yx, xx), each sum ab / n - c_a c_b;
+ * each float64 step one correctly rounded operation, 0.0 for an empty node.  No scratch; asynchronous on `stream`, never
+ * synchronises (a CUDA graph can capture it); batch == 0 does nothing, D, H or W == 0 zeroes the outputs. */
+int fslic_b200_props3d_batch(int device, int batch, int D, int H, int W, int K, const uint16_t* d_labels,
+                             int32_t* d_area, int32_t* d_bbox, long long* d_moments, long long* d_surface,
+                             int32_t* d_border, double* d_centroid, double* d_covariance, void* stream);
 
 /* Superpixels merged into regions (merge.cuh; no counterpart in the reference): single-linkage cuts of a region
  * adjacency graph over `batch` label maps d_labels u16[B,H,W].  Node n = b*K + k is label k of image b, present when a
