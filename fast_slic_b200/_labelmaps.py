@@ -71,6 +71,12 @@ def check_pixels(H, W, reason=""):
         raise ValueError("images of %dx%d pixels exceed %d pixels%s" % (H, W, MAX_PIXELS, reason))
 
 
+def check_voxels(D, H, W, reason=""):
+    """Volumes of at most MAX_PIXELS voxels; `reason` ends the message."""
+    if D * H * W > MAX_PIXELS:
+        raise ValueError("volumes of %dx%dx%d voxels exceed %d voxels%s" % (D, H, W, MAX_PIXELS, reason))
+
+
 def check_features(labels, name, x, ndim):
     """labels int16 [B,H,W] and x float32 with ndim dimensions, same B (and H, W for ndim 4); returns (B, H, W, C)."""
     tensor("labels", labels, torch.int16, 3)

@@ -43,11 +43,14 @@ EXPORTED_SYMBOLS = (
     "fslic_b200_rag_batch_fill", "fslic_b200_rag3d_batch_scratch_bytes", "fslic_b200_rag3d_batch_count",
     "fslic_b200_rag3d_batch_fill",
     "fslic_b200_gt_histogram_batch", "fslic_b200_gt_scores_scratch_bytes", "fslic_b200_gt_scores_batch",
-    "fslic_b200_gt_boundaries_batch",
+    "fslic_b200_gt_boundaries_batch", "fslic_b200_gt_scores3d_scratch_bytes", "fslic_b200_gt_scores3d_batch",
+    "fslic_b200_gt_boundaries3d_batch",
     "fslic_b200_props_batch", "fslic_b200_props3d_batch",
     "fslic_b200_merge_scratch_bytes", "fslic_b200_merge_batch",
     "fslic_b200_boundary_select_scratch_bytes", "fslic_b200_boundary_select_batch",
     "fslic_b200_boundary_stats_scratch_bytes", "fslic_b200_boundary_stats_batch",
+    "fslic_b200_boundary3d_select_scratch_bytes", "fslic_b200_boundary3d_select_batch",
+    "fslic_b200_boundary3d_stats_scratch_bytes", "fslic_b200_boundary3d_stats_batch",
     "fslic_b200_knn_scratch_bytes", "fslic_b200_knn_count", "fslic_b200_knn_fill",
     "fslic_b200_feature_slic_scratch_bytes", "fslic_b200_feature_slic",
     "fslic_b200_soft_assign", "fslic_b200_soft_assign_backward", "fslic_b200_soft_pool",
@@ -160,6 +163,10 @@ def lib():
     L.fslic_b200_gt_scores_batch.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, i32, i64, vp, vp, C.c_size_t,
                                              vp]
     L.fslic_b200_gt_boundaries_batch.argtypes = [i32, i32, i32, i32, vp, vp, vp]
+    L.fslic_b200_gt_scores3d_scratch_bytes.argtypes = [i32] * 5
+    L.fslic_b200_gt_scores3d_scratch_bytes.restype = C.c_size_t
+    L.fslic_b200_gt_scores3d_batch.argtypes = [i32] * 10 + [vp, vp, i32, i64, vp, vp, C.c_size_t, vp]
+    L.fslic_b200_gt_boundaries3d_batch.argtypes = [i32] * 5 + [vp] * 3
     L.fslic_b200_props_batch.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.fslic_b200_props3d_batch.argtypes = [i32] * 6 + [vp] * 9
     L.fslic_b200_merge_scratch_bytes.argtypes = [i32, i32]
@@ -173,6 +180,13 @@ def lib():
     L.fslic_b200_boundary_stats_scratch_bytes.restype = C.c_size_t
     L.fslic_b200_boundary_stats_batch.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, i64, vp, C.c_size_t, i64,
                                                   i64, i64, vp, vp, i32, vp, vp, vp, vp, vp, C.c_size_t, vp]
+    L.fslic_b200_boundary3d_select_scratch_bytes.argtypes = [i32] * 6
+    L.fslic_b200_boundary3d_select_scratch_bytes.restype = C.c_size_t
+    L.fslic_b200_boundary3d_select_batch.argtypes = [i32] * 7 + [vp, vp, vp, C.c_size_t, vp]
+    L.fslic_b200_boundary3d_stats_scratch_bytes.argtypes = [i64] * 3
+    L.fslic_b200_boundary3d_stats_scratch_bytes.restype = C.c_size_t
+    L.fslic_b200_boundary3d_stats_batch.argtypes = [i32] * 8 + [vp, vp, i64, i64, vp, C.c_size_t, i64, i64, i64, vp, vp,
+                                                                i32, vp, vp, vp, vp, vp, C.c_size_t, vp]
     L.fslic_b200_knn_scratch_bytes.argtypes = [i32, i32, i32, i32, i32]
     L.fslic_b200_knn_scratch_bytes.restype = C.c_size_t
     L.fslic_b200_knn_count.argtypes = [i32, i32, i32, i32, i32, i32, vp, vp, i64, vp, vp, vp, C.c_size_t, vp]

@@ -221,3 +221,169 @@ __global__ void __launch_bounds__(256) k_boundary_runs(const unsigned long long*
         }
     }
 }
+
+// ---- Volumes (DESIGN.md section 4.24): label volumes u16 [batch, D, H, W] and values f32 [batch, C, D, H, W], the
+// voxel pairs of region adjacency (rag.cuh's k_rag3d_discover): each voxel (the anchor) with its forward neighbours
+// (dz, dy, dx) of BOUNDARY3D_DIRS, the first 3 (connectivity 6), 9 (18) or 13 (26).  Pair ordinal = anchor * Ndir + d.
+// The selection is sized per voxel, not per voxel pair:
+//   select      k_boundary3d_mask     a 13-bit mask of each voxel's boundary directions (2 bytes per voxel);
+//               (cub::DeviceSelect::Flagged of the voxels with a mask, in voxel order, 4 bytes per voxel, and
+//               cub::DeviceReduce::Sum of popc(mask): the caller reads back the voxel count and the pair count)
+//   stats       (cub::DeviceScan::ExclusiveSum of popc(mask) over the selected voxels: each voxel's first pair)
+//               k_boundary3d_expand   one record per boundary pair in ordinal order: key, position, anchor, direction;
+//               (stable radix sort of the keys, the position as the value; then the 2-D heads, run starts and entry
+//               keys above)
+//               k_boundary3d_runs     k_boundary_runs with the other voxel at anchor + off[d].
+// Every forward offset dz * H * W + dy * W + dx of a pair that exists is positive.
+struct Boundary3dDirs {
+    int off[13];  // dz * H * W + dy * W + dx of each direction, host-built for the call's H, W
+};
+
+__device__ __forceinline__ int boundary3d_dir(int d, int a) {
+    constexpr int8_t dirs[13][3] = {{0, 0, 1}, {0, 1, 0},  {1, 0, 0},  {0, 1, 1},  {0, 1, -1},
+                                    {1, 1, 0}, {1, -1, 0}, {1, 0, 1},  {1, 0, -1}, {1, 1, 1},
+                                    {1, 1, -1}, {1, -1, 1}, {1, -1, -1}};
+    return dirs[d][a];
+}
+
+// mask[t] = bit d set where voxel t's pair in direction d exists, both labels are in [0, K) and they differ
+template <int NDIR>
+__global__ void __launch_bounds__(256) k_boundary3d_mask(const uint16_t* __restrict__ lab, uint32_t dhw, int D, int H,
+                                                          int W, uint32_t n, int K, Boundary3dDirs dirs,
+                                                          uint16_t* __restrict__ mask) {
+    const uint32_t hw = (uint32_t)H * (uint32_t)W;
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
+        const uint32_t p = t % dhw, z = p / hw, r = p - z * hw, y = r / (uint32_t)W, x = r - y * (uint32_t)W;
+        const uint32_t s = lab[t];
+        uint32_t m = 0;
+        if (s < (uint32_t)K) {
+#pragma unroll
+            for (int d = 0; d < NDIR; d++) {
+                const int dz = boundary3d_dir(d, 0), dy = boundary3d_dir(d, 1), dx = boundary3d_dir(d, 2);
+                if ((int)z + dz < D && (int)y + dy >= 0 && (int)y + dy < H && (int)x + dx >= 0 && (int)x + dx < W) {
+                    const uint32_t g = lab[t + dirs.off[d]];
+                    if (g < (uint32_t)K && g != s) m |= 1u << d;
+                }
+            }
+        }
+        mask[t] = (uint16_t)m;
+    }
+}
+
+// counts[0] = the selected voxel count (the pair sum writes counts[1])
+__global__ void k_boundary3d_count(const int* __restrict__ nsel, long long* __restrict__ counts) { counts[0] = *nsel; }
+
+// popc of the mask of selected voxel i
+struct Boundary3dPopc {
+    const uint16_t* mask;
+    const uint32_t* sel;
+    __device__ __forceinline__ uint32_t operator()(uint32_t i) const { return (uint32_t)__popc(mask[sel[i]]); }
+};
+
+// popc of the mask of voxel t, 64-bit: the pair count of a call can exceed 2^32
+struct Boundary3dPopc64 {
+    const uint16_t* mask;
+    __device__ __forceinline__ unsigned long long operator()(uint32_t t) const {
+        return (unsigned long long)__popc(mask[t]);
+    }
+};
+
+// Selected voxel i (first pair first[i]): for each of its boundary directions d in increasing order, the record at
+// q = first[i] + j: key (image << 32 | lo << 16 | hi), pos = q, anchor = the voxel, dir = d
+__global__ void __launch_bounds__(256) k_boundary3d_expand(const uint32_t* __restrict__ sel, uint32_t voxels,
+                                                            const uint16_t* __restrict__ mask,
+                                                            const uint32_t* __restrict__ first,
+                                                            const uint16_t* __restrict__ lab, uint32_t dhw,
+                                                            Boundary3dDirs dirs, unsigned long long* __restrict__ key,
+                                                            uint32_t* __restrict__ pos, uint32_t* __restrict__ anchor,
+                                                            uint8_t* __restrict__ dir) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < voxels; i += gridDim.x * blockDim.x) {
+        const uint32_t t = sel[i], a = lab[t];
+        const unsigned long long image = (unsigned long long)(t / dhw) << 32;
+        uint32_t m = mask[t], q = first[i];
+        while (m) {
+            const int d = __ffs(m) - 1;
+            m &= m - 1;
+            const uint32_t g = lab[t + dirs.off[d]];
+            key[q] = image | (a < g ? a << 16 | g : g << 16 | a);
+            pos[q] = q;
+            anchor[q] = t;
+            dir[q] = (uint8_t)d;
+            q++;
+        }
+    }
+}
+
+// k_boundary_runs for volumes: run r of *d_runs is sorted positions [start[r], start[r + 1] or pairs); pair spos[i]
+// has its anchor voxel anchor[.] and the other voxel anchor + off[dir[.]].  values [batch, C, dhw].
+__global__ void __launch_bounds__(256) k_boundary3d_runs(const unsigned long long* __restrict__ skey,
+                                                          const uint32_t* __restrict__ spos,
+                                                          const uint32_t* __restrict__ anchor,
+                                                          const uint8_t* __restrict__ dir,
+                                                          const uint32_t* __restrict__ start,
+                                                          const int* __restrict__ d_runs, int pairs,
+                                                          const unsigned long long* __restrict__ sekey,
+                                                          const uint32_t* __restrict__ seidx, int edges,
+                                                          const float* __restrict__ values, int C, uint32_t dhw,
+                                                          Boundary3dDirs dirs, float* __restrict__ mean,
+                                                          float* __restrict__ mn, float* __restrict__ mx,
+                                                          int32_t* __restrict__ count) {
+    const int lane = threadIdx.x & 31;
+    const long nwarps = ((long)gridDim.x * blockDim.x) >> 5;
+    const int runs = *d_runs;
+    for (long r = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < runs; r += nwarps) {
+        const int s = (int)start[r], e = r + 1 < runs ? (int)start[r + 1] : pairs;
+        const unsigned long long key = skey[s];
+        int pos = 0;
+        if (lane < 2) pos = boundary_lower_bound(sekey, edges, key + (unsigned long long)lane);
+        const int m0 = __shfl_sync(FSLIC_FULL, pos, 0), m = __shfl_sync(FSLIC_FULL, pos, 1) - m0;
+        if (m == 0) continue;
+        const uint32_t n = (uint32_t)(e - s), nv = 2 * n;
+        const float f2n = __uint2float_rn(nv);
+        const uint32_t base = (uint32_t)(key >> 32) * dhw;
+        const float* f = values + (long)(key >> 32) * C * dhw;
+        for (int k = lane; k < m; k += 32) count[seidx[m0 + k]] = (int32_t)n;
+        int c = 0;
+        for (; c + 4 <= C; c += 4) {
+            const float* fc = f + (long)c * dhw;
+            float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+            int lo[4] = {INT_MAX, INT_MAX, INT_MAX, INT_MAX}, hi[4] = {INT_MIN, INT_MIN, INT_MIN, INT_MIN};
+            bool nan[4] = {false, false, false, false};
+            for (uint32_t j = lane; j < nv; j += 32) {
+                const uint32_t q = spos[s + (j >> 1)];
+                const uint32_t p = anchor[q] - base + ((j & 1) ? (uint32_t)dirs.off[dir[q]] : 0u);
+#pragma unroll
+                for (int u = 0; u < 4; u++) boundary_add(__ldg(fc + (long)u * dhw + p), acc[u], lo[u], hi[u], nan[u]);
+            }
+            float rm[4], ra[4], rb[4];
+#pragma unroll
+            for (int u = 0; u < 4; u++) boundary_finish(acc[u], lo[u], hi[u], nan[u], f2n, &rm[u], &ra[u], &rb[u]);
+            for (int q = lane; q < 4 * m; q += 32) {
+                const int u = q & 3;
+                const long o = (long)seidx[m0 + (q >> 2)] * C + c + u;
+                mean[o] = u == 0 ? rm[0] : u == 1 ? rm[1] : u == 2 ? rm[2] : rm[3];
+                mn[o] = u == 0 ? ra[0] : u == 1 ? ra[1] : u == 2 ? ra[2] : ra[3];
+                mx[o] = u == 0 ? rb[0] : u == 1 ? rb[1] : u == 2 ? rb[2] : rb[3];
+            }
+        }
+        for (; c < C; c++) {
+            const float* fc = f + (long)c * dhw;
+            float acc = 0.0f;
+            int lo = INT_MAX, hi = INT_MIN;
+            bool nan = false;
+            for (uint32_t j = lane; j < nv; j += 32) {
+                const uint32_t q = spos[s + (j >> 1)];
+                const uint32_t p = anchor[q] - base + ((j & 1) ? (uint32_t)dirs.off[dir[q]] : 0u);
+                boundary_add(__ldg(fc + p), acc, lo, hi, nan);
+            }
+            float rm, ra, rb;
+            boundary_finish(acc, lo, hi, nan, f2n, &rm, &ra, &rb);
+            for (int k = lane; k < m; k += 32) {
+                const long o = (long)seidx[m0 + k] * C + c;
+                mean[o] = rm;
+                mn[o] = ra;
+                mx[o] = rb;
+            }
+        }
+    }
+}

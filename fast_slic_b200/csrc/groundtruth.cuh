@@ -267,3 +267,155 @@ __global__ void __launch_bounds__(256) k_gt_boundaries(const uint16_t* __restric
         out[t] = gt_sp_boundary(lab, t, i, j, H, W) ? 1 : 0;
     }
 }
+
+// ---- Volumes (DESIGN.md section 4.24): label volumes u16 [batch, D, H, W] and gt of the same shape.  The overlap keys
+// are k_gt_keys' over D * H * W voxels per volume; the boundary terms use 3-D one-sided boundaries and a box window
+// |dz| <= rz, |dy| <= ry, |dx| <= rx, dilated separably:
+//   k_gt_bitmaps3d        k_gt_bitmaps with the +z neighbour too, over the D * H rows of each volume;
+//   k_gt_dilate_yx        one thread per word: the superpixel and gt boundary bitmaps ORed over rows i - ry .. i + ry
+//                         of the word's slice and three words, dilated by rx within them;
+//   k_gt_boundary_counts3d  one thread per word: those ORed over slices z - rz .. z + rz, then k_gt_boundary_counts'
+//                         four popc counts, warp sums and int64 atomicAdds.
+
+// Voxel (z, i, j) of a volume is a supervoxel boundary voxel when its +x, +y or +z neighbour exists and carries another
+// raw label.  p is the voxel's offset in the volume, hw = H * W.
+__device__ __forceinline__ bool gt_sp_boundary3d(const uint16_t* __restrict__ lab, long p, int z, int i, int j, int D,
+                                                 int H, int W, long hw) {
+    const uint16_t s = lab[p];
+    return (j + 1 < W && lab[p + 1] != s) || (i + 1 < H && lab[p + W] != s) || (z + 1 < D && lab[p + hw] != s);
+}
+
+// Bitmaps [batch][D][H][Wd] as k_gt_bitmaps' (sp, gb, gv), with 3-D boundaries.  Grid: y over volumes, x over the
+// D * H * Wd * 32 columns of a volume, one warp per word.
+template <typename T>
+__global__ void __launch_bounds__(256) k_gt_bitmaps3d(const uint16_t* __restrict__ lab, const T* __restrict__ gt,
+                                                       int batch, int D, int H, int W, int Wd, int has_ignore,
+                                                       long long ignore, uint32_t* __restrict__ sp,
+                                                       uint32_t* __restrict__ gb, uint32_t* __restrict__ gv) {
+    // D * H * Wd < 2^32 for D * H * W <= 2^29: 32-bit word indices
+    const uint32_t words = (uint32_t)D * (uint32_t)H * (uint32_t)Wd;
+    const long hw = (long)H * W, dhw = (long)D * hw;
+    const uint32_t warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, wstep = (gridDim.x * blockDim.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    for (long b = blockIdx.y; b < batch; b += gridDim.y) {
+        const uint16_t* l = lab + b * dhw;
+        const T* g = gt + b * dhw;
+        for (uint32_t q = warp0; q < words; q += wstep) {
+            const uint32_t row = q / (uint32_t)Wd, w = q - row * (uint32_t)Wd;
+            const int z = (int)(row / (uint32_t)H), i = (int)(row - (uint32_t)z * (uint32_t)H), j = (int)w * 32 + lane;
+            bool s = false, e = false, ok = false;
+            if (j < W) {
+                const long p = (long)row * W + j;
+                s = gt_sp_boundary3d(l, p, z, i, j, D, H, W, hw);
+                const T x = g[p];
+                ok = gt_valid(x, has_ignore, ignore);
+                if (ok) {
+                    if (j + 1 < W) {
+                        const T y = g[p + 1];
+                        e = gt_valid(y, has_ignore, ignore) && y != x;
+                    }
+                    if (!e && i + 1 < H) {
+                        const T y = g[p + W];
+                        e = gt_valid(y, has_ignore, ignore) && y != x;
+                    }
+                    if (!e && z + 1 < D) {
+                        const T y = g[p + hw];
+                        e = gt_valid(y, has_ignore, ignore) && y != x;
+                    }
+                }
+            }
+            const uint32_t ws = __ballot_sync(FSLIC_FULL, s), we = __ballot_sync(FSLIC_FULL, e),
+                           wv = __ballot_sync(FSLIC_FULL, ok);
+            if (lane == 0) {
+                const long o = b * (long)words + q;
+                sp[o] = ws;
+                gb[o] = we;
+                gv[o] = wv;
+            }
+        }
+    }
+}
+
+// ds / de = sp / gb dilated within each slice: bit c of word (z, i, w) is set when a bit of rows i - ry .. i + ry
+// (clipped to the slice) and columns c - rx .. c + rx is.  Grid: y over volumes, x over the D * H * Wd words.
+__global__ void __launch_bounds__(256) k_gt_dilate_yx(const uint32_t* __restrict__ sp, const uint32_t* __restrict__ gb,
+                                                       int batch, int D, int H, int Wd, int ry, int rx,
+                                                       uint32_t* __restrict__ ds, uint32_t* __restrict__ de) {
+    const uint32_t words = (uint32_t)D * (uint32_t)H * (uint32_t)Wd;
+    for (long b = blockIdx.y; b < batch; b += gridDim.y) {
+        const uint32_t* s = sp + b * (long)words;
+        const uint32_t* e = gb + b * (long)words;
+        for (uint32_t q = blockIdx.x * blockDim.x + threadIdx.x; q < words; q += gridDim.x * blockDim.x) {
+            const uint32_t row = q / (uint32_t)Wd, w = q - row * (uint32_t)Wd;
+            const uint32_t z = row / (uint32_t)H;
+            const int i = (int)(row - z * (uint32_t)H);
+            const int i0 = i - ry < 0 ? 0 : i - ry, i1 = i + ry >= H ? H - 1 : i + ry;
+            const uint32_t slice = z * (uint32_t)H * (uint32_t)Wd;
+            uint32_t vs[3] = {0, 0, 0}, ve[3] = {0, 0, 0};
+            for (int ii = i0; ii <= i1; ii++) {
+                const uint32_t r0 = slice + (uint32_t)ii * (uint32_t)Wd + w;
+                if (w > 0) {
+                    vs[0] |= s[r0 - 1];
+                    ve[0] |= e[r0 - 1];
+                }
+                vs[1] |= s[r0];
+                ve[1] |= e[r0];
+                if (w + 1 < (uint32_t)Wd) {
+                    vs[2] |= s[r0 + 1];
+                    ve[2] |= e[r0 + 1];
+                }
+            }
+            ds[b * (long)words + q] = gt_hdilate(vs[0], vs[1], vs[2], rx);
+            de[b * (long)words + q] = gt_hdilate(ve[0], ve[1], ve[2], rx);
+        }
+    }
+}
+
+// out[b][GT_BOUNDARY .. GT_SP_BOUNDARY_HITS] += k_gt_boundary_counts' four terms, the windows being ds / de ORed over
+// slices z - rz .. z + rz (clipped to the volume).  Grid: y over volumes, x over the D * H * Wd words.
+__global__ void __launch_bounds__(256) k_gt_boundary_counts3d(const uint32_t* __restrict__ sp,
+                                                               const uint32_t* __restrict__ gb,
+                                                               const uint32_t* __restrict__ gv,
+                                                               const uint32_t* __restrict__ ds,
+                                                               const uint32_t* __restrict__ de, int batch, int D,
+                                                               int H, int Wd, int rz, long long* __restrict__ out) {
+    const uint32_t plane = (uint32_t)H * (uint32_t)Wd, words = (uint32_t)D * plane;
+    for (long b = blockIdx.y; b < batch; b += gridDim.y) {
+        const long o = b * (long)words;
+        uint32_t c[4] = {0, 0, 0, 0};
+        for (uint32_t q = blockIdx.x * blockDim.x + threadIdx.x; q < words; q += gridDim.x * blockDim.x) {
+            const int z = (int)(q / plane);
+            const uint32_t r = q - (uint32_t)z * plane;
+            const int z0 = z - rz < 0 ? 0 : z - rz, z1 = z + rz >= D ? D - 1 : z + rz;
+            uint32_t ws = 0, we = 0;
+            for (int zz = z0; zz <= z1; zz++) {
+                ws |= ds[o + (uint32_t)zz * plane + r];
+                we |= de[o + (uint32_t)zz * plane + r];
+            }
+            const uint32_t own_s = sp[o + q] & gv[o + q], own_e = gb[o + q];
+            c[0] += __popc(own_e);
+            c[1] += __popc(own_e & ws);
+            c[2] += __popc(own_s);
+            c[3] += __popc(own_s & we);
+        }
+        // at most D * H * W <= 2^29 per volume and term: the warp sums fit u32
+#pragma unroll
+        for (int f = 0; f < 4; f++) {
+            const uint32_t t = __reduce_add_sync(FSLIC_FULL, c[f]);
+            if ((threadIdx.x & 31) == 0 && t)
+                atomicAdd(reinterpret_cast<unsigned long long*>(&out[b * GT_FIELDS + GT_BOUNDARY + f]),
+                          (unsigned long long)t);
+        }
+    }
+}
+
+// out[t] = 1 where voxel t is a supervoxel boundary voxel, else 0
+__global__ void __launch_bounds__(256) k_gt_boundaries3d(const uint16_t* __restrict__ lab, uint32_t dhw, int D, int H,
+                                                          int W, long n, uint8_t* __restrict__ out) {
+    const uint32_t hw = (uint32_t)H * (uint32_t)W;
+    for (long t = (long)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += (long)gridDim.x * blockDim.x) {
+        const uint32_t p = (uint32_t)(t - gt_image(t, dhw, n) * (long)dhw);  // dhw <= 2^29: 32-bit divisions
+        const uint32_t z = p / hw, r = p - z * hw, i = r / (uint32_t)W, j = r - i * (uint32_t)W;
+        out[t] = gt_sp_boundary3d(lab, t, (int)z, (int)i, (int)j, D, H, W, (long)hw) ? 1 : 0;
+    }
+}

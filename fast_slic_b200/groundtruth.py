@@ -14,18 +14,19 @@ region_graph.region_adjacency it gives a superpixel GNN its targets::
 read as uint16, and a class / gt map of the same shape, uint8, int16, int32 or int64.  Every argument is checked
 (ValueError) before any device work.  Work runs on the labels' device, on its current stream, and nothing is read back
 to the host, so a CUDA graph can capture every call.  All arithmetic is integer: image b's result depends only on
-labels[b] and gt[b] -- not on the batch, its place in it, the chunking, the stream or the run.  DESIGN.md section 4.14
-describes the kernels.
+labels[b] and gt[b] -- not on the batch, its place in it, the chunking, the stream or the run.  segmentation_scores_3d
+and boundaries_3d are the same for label volumes [B,D,H,W], with 3-D boundaries and a box tolerance window that can
+differ per axis.  DESIGN.md sections 4.14 and 4.24 describe the kernels.
 """
 import collections
 
 import torch
 
 from . import _lib
-from ._labelmaps import NO_SIZE, check_int, check_K, check_pixels, chunk, cuda_device, tensor
+from ._labelmaps import NO_SIZE, check_int, check_K, check_pixels, check_voxels, chunk, cuda_device, tensor
 
-# Device memory one scores launch takes at most (about 20.4 bytes per pixel and 16 per superpixel, plus the sort's
-# storage): a batch that needs more runs in chunks of images, with identical results.
+# Device memory one scores launch takes at most (about 20.4 bytes per pixel, 20.6 per voxel, and 16 per superpixel,
+# plus the sort's storage): a batch that needs more runs in chunks of images or volumes, with identical results.
 GT_SCRATCH_CAP = 1 << 30
 MAX_CLASSES = 65536
 MAX_TOLERANCE = 32
@@ -39,19 +40,22 @@ SegmentationScores = collections.namedtuple("SegmentationScores", [
     "asa", "undersegmentation", "boundary_recall", "boundary_precision"])
 
 
-def _check(name, gt, labels):
-    """labels: int16 [B,H,W]; gt: a [B,H,W] map of a _DTYPES dtype; images of at most MAX_PIXELS pixels.  Returns
-    (B, H, W)."""
-    tensor("labels", labels, torch.int16, 3)
+def _check(name, gt, labels, ndim=3):
+    """labels: int16 [B,H,W] (ndim 3) or [B,D,H,W] (ndim 4); gt: a map of the same shape and a _DTYPES dtype; images
+    or volumes of at most MAX_PIXELS pixels.  Returns the shape."""
+    tensor("labels", labels, torch.int16, ndim)
     if not isinstance(gt, torch.Tensor):
         raise ValueError("%s must be a cuda tensor (got %s): use torch.from_numpy(...).cuda()" % (name, type(gt).__name__))
     if gt.dtype not in _DTYPES:
         raise ValueError("%s must be a uint8, int16, int32 or int64 tensor, got %s" % (name, gt.dtype))
     if tuple(gt.shape) != tuple(labels.shape):
         raise ValueError("%s %s does not match labels %s" % (name, tuple(gt.shape), tuple(labels.shape)))
-    B, H, W = (int(v) for v in labels.shape)
-    check_pixels(H, W, ": a count could overflow int32")
-    return B, H, W
+    shape = tuple(int(v) for v in labels.shape)
+    if ndim == 4:
+        check_voxels(*shape[1:], ": a count could overflow int32")
+    else:
+        check_pixels(*shape[1:], ": a count could overflow int32")
+    return shape
 
 
 def class_histogram(classes, labels, K, num_classes):
@@ -153,4 +157,76 @@ def boundaries(labels):
             lab = labels.contiguous()
             _lib.check(_lib.lib().fslic_b200_gt_boundaries_batch(dev.index, B, H, W, lab.data_ptr(), out.data_ptr(),
                                                                  torch.cuda.current_stream(dev).cuda_stream))
+    return out
+
+
+def gt3d_chunk(B, D, H, W, K):
+    """Volumes per scores launch of segmentation_scores_3d: as many as fit GT_SCRATCH_CAP, at least one."""
+    f = _lib.lib().fslic_b200_gt_scores3d_scratch_bytes
+    if f(1, D, H, W, K) == NO_SIZE:
+        raise ValueError("a volume of %dx%dx%d voxels is too large to score" % (D, H, W))
+    return chunk(lambda c: f(c, D, H, W, K), GT_SCRATCH_CAP, B, limit=_MAX_CHUNK)
+
+
+def check_tolerance_3d(tolerance):
+    """An int r in [0, 32] -> (r, r, r); a tuple or list (rz, ry, rx) of such ints -> itself as a tuple."""
+    if isinstance(tolerance, (tuple, list)):
+        if len(tolerance) != 3:
+            raise ValueError("tolerance must be an int or a (rz, ry, rx) tuple, got %r" % (tolerance,))
+        return tuple(check_int("tolerance", r, 0, MAX_TOLERANCE) for r in tolerance)
+    r = check_int("tolerance", tolerance, 0, MAX_TOLERANCE)
+    return r, r, r
+
+
+def segmentation_scores_3d(labels, gt, K, tolerance=2, ignore_index=None):
+    """Scores of int16 supervoxel labels [B,D,H,W] (read as uint16) against a ground-truth segmentation gt [B,D,H,W]
+    (uint8, int16, int32 or int64) -> SegmentationScores, every field a [B] tensor: segmentation_scores for volumes.
+    - pixels, asa_pixels, ue_pixels and their ratios count voxels and equal segmentation_scores on the [B, D*H, W]
+      views of labels and gt (the overlap table does not depend on the layout).
+    - The boundaries are 3-D and one-sided: a supervoxel boundary voxel is one of boundaries_3d, a gt boundary voxel
+      is valid and has a valid +x, +y or +z neighbour with another value; sp_boundary counts the supervoxel boundary
+      voxels valid in gt.
+    - The window of a voxel is the box |dz| <= rz, |dy| <= ry, |dx| <= rx clipped to the volume.  tolerance is an int
+      r in [0, 32] (rz = ry = rx = r) or a tuple (rz, ry, rx) of such ints, for anisotropic voxels such as CT's thick
+      slices.
+    At D = 1 every field equals segmentation_scores on labels[:, 0] with the tolerance ry = rx.  The call reads nothing
+    back, so a CUDA graph can capture it; volumes run in chunks under GT_SCRATCH_CAP with identical results."""
+    B, D, H, W = _check("gt", gt, labels, 4)
+    K = check_K(K)
+    rz, ry, rx = check_tolerance_3d(tolerance)
+    ignore = None if ignore_index is None else check_int("ignore_index", ignore_index, *_INT64)
+    dev = cuda_device(labels, ("gt", gt))
+    with torch.cuda.device(dev):
+        out = torch.zeros((B, 7), dtype=torch.int64, device=dev)
+        if B and D and H and W:
+            g, lab = gt.contiguous(), labels.contiguous()
+            L = _lib.lib()
+            chunk = gt3d_chunk(B, D, H, W, K)
+            nbytes = int(L.fslic_b200_gt_scores3d_scratch_bytes(chunk, D, H, W, K))
+            scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            for b0 in range(0, B, chunk):
+                c = min(chunk, B - b0)
+                _lib.check(L.fslic_b200_gt_scores3d_batch(
+                    dev.index, c, D, H, W, K, rz, ry, rx, _DTYPES[g.dtype], g[b0].data_ptr(), lab[b0].data_ptr(),
+                    int(ignore is not None), 0 if ignore is None else ignore, out[b0].data_ptr(), scratch.data_ptr(),
+                    nbytes, stream))
+        f = out.t().contiguous().unbind(0)
+        return SegmentationScores(*f, _ratio(f[1], f[0]), _ratio(f[2], f[0]), _ratio(f[4], f[3]), _ratio(f[6], f[5]))
+
+
+def boundaries_3d(labels):
+    """int16 labels [B,D,H,W] -> bool [B,D,H,W]: True at supervoxel boundary voxels, those whose +x, +y or +z neighbour
+    exists and carries another raw label -- a one-sided, 1-voxel-wide outline, the predicate segmentation_scores_3d
+    uses.  No scratch and no read-back: a CUDA graph can capture it."""
+    tensor("labels", labels, torch.int16, 4)
+    B, D, H, W = (int(v) for v in labels.shape)
+    check_voxels(D, H, W)
+    dev = cuda_device(labels)
+    with torch.cuda.device(dev):
+        out = torch.empty((B, D, H, W), dtype=torch.bool, device=dev)
+        if B and D and H and W:
+            lab = labels.contiguous()
+            _lib.check(_lib.lib().fslic_b200_gt_boundaries3d_batch(dev.index, B, D, H, W, lab.data_ptr(), out.data_ptr(),
+                                                                   torch.cuda.current_stream(dev).cuda_stream))
     return out

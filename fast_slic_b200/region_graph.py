@@ -21,8 +21,9 @@ by the lower index, in the same node numbering and CSR layout::
 
 No counterpart in the reference: its get_connectivity keeps at most 12 neighbours per superpixel, in scan order, and
 is kept for parity with it; its get_knn_connectivity has no defined result and raises NotImplementedError here.
-region_adjacency_3d is the graph of supervoxel label volumes [B,D,H,W], in 6-, 18- or 26-connectivity.  DESIGN.md
-sections 4.13, 4.17, 4.18 and 4.23 describe the kernels.
+region_adjacency_3d is the graph of supervoxel label volumes [B,D,H,W], in 6-, 18- or 26-connectivity, and
+boundary_stats_3d the statistics of voxel maps along its faces.  DESIGN.md sections 4.13, 4.17, 4.18, 4.23 and 4.24
+describe the kernels.
 """
 import collections
 
@@ -31,7 +32,7 @@ import torch
 
 from . import _lib
 from ._labelmaps import (MAX_PIXELS, NO_SIZE, check_connectivity, check_connectivity_3d, check_features, check_graph,
-                         check_int, check_K, check_pixels, chunk, cuda_device, tensor)
+                         check_int, check_K, check_pixels, check_voxels, chunk, cuda_device, tensor)
 
 # Device memory the pair tables of one count launch take at most (8 bytes per slot, a power of two >= max(4096, 32 K)
 # slots per image): a batch that needs more runs in chunks of images, with identical results.
@@ -40,6 +41,8 @@ RAG_SCRATCH_CAP = 1 << 30
 # sized before the pair count is known: a batch that needs more runs in chunks of images, with identical results.  A
 # chunk whose boundary pairs need more than this for their sort is split again (only maps that are not superpixel maps,
 # such as noise, have that many).
+# boundary_stats_3d takes the same cap for its selection, which takes 6 bytes per voxel (so a 256x512x512 volume fits
+# at any connectivity), and halves a chunk in the same way.
 BOUNDARY_SCRATCH_CAP = 1 << 30
 # Device memory one kNN launch takes at most (about 17 + 4 D + 8 k bytes per node, 72 k more for a symmetric graph):
 # a batch that needs more runs in chunks of images, with identical results.
@@ -312,6 +315,101 @@ def boundary_stats(labels, K, graph, values, connectivity=4):
             scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
             _lib.check(L.fslic_b200_boundary_stats_batch(
                 dev.index, c, H, W, K, C, connectivity, lab[b0].data_ptr(), val[b0].data_ptr(), pairs,
+                select.data_ptr(), nbytes, b0, B * K, E, ei[0].data_ptr(), ei[1].data_ptr(), first,
+                out.mean.data_ptr(), out.min.data_ptr(), out.max.data_ptr(), out.count.data_ptr(), scratch.data_ptr(),
+                sbytes, stream))
+            first = 0
+    return out
+
+
+def boundary3d_chunk(B, D, H, W, K, connectivity):
+    """Volumes per boundary voxel selection of boundary_stats_3d: as many as fit BOUNDARY_SCRATCH_CAP, at least one."""
+    f = _lib.lib().fslic_b200_boundary3d_select_scratch_bytes
+    if f(1, D, H, W, K, connectivity) == NO_SIZE:
+        raise ValueError("a volume of %dx%dx%d voxels is too large for boundary statistics" % (D, H, W))
+    return chunk(lambda c: f(c, D, H, W, K, connectivity), BOUNDARY_SCRATCH_CAP, B)
+
+
+def boundary_stats_3d(labels, K, graph, values, connectivity=6):
+    """Statistics of voxel maps along the shared boundary of every entry of a region adjacency graph of label volumes
+    -> BoundaryStats(mean, min, max, count), detached: boundary_stats for volumes, with the same outputs, float32
+    [E, C] and int32 [E], and the same rules.  labels is a cuda int16 [B,D,H,W] tensor (read as uint16), values float32
+    [B,C,D,H,W] (C >= 1) on the same device.  graph is a RegionGraph (region_adjacency_3d(labels, K, connectivity)) or
+    any object with indptr of B*K + 1 entries and int64 edge_index [2,E]; only edge_index is read.
+
+    Voxel pairs are region_adjacency_3d's: each voxel (the anchor) with its forward neighbours RAG3D_OFFSETS[:3]
+    (connectivity 6), [:9] (18) or [:13] (26); a pair's ordinal is anchor_index * Ndir + d, d its index in
+    RAG3D_OFFSETS.  A boundary pair has both labels in [0, K) and different.  Entry e = (u, v) of volume b gets the
+    boundary pairs whose labels are {u % K, v % K}; the 2n values of an entry, per channel, are values[b, c, anchor]
+    then values[b, c, other] of each pair in increasing ordinal; mean is their sum in pool's lane order divided by
+    (float)(2n); min / max follow the total order of non-NaN floats with -0.0 < +0.0, NaN when any value is NaN.  An
+    entry with no pairs, across volumes, out of range or with equal endpoints gets NaN and count 0 and never faults.
+    For a graph from region_adjacency_3d with the same labels and connectivity, count equals graph.boundary.  At D = 1
+    the result equals boundary_stats on labels[:, 0] with connectivity 4 (for 6) or 8 (for 18 and 26).
+
+    ValueError, before any device work, for: labels that are not a cuda int16 [B,D,H,W] tensor, values that are not
+    float32 [B,C,D,H,W] with the labels' B, D, H, W and C >= 1, K outside [1, 65534], volumes over 2^29 voxels or with
+    more than 2^31 - 1 voxel pairs (voxel_pairs), connectivity other than 6, 18 or 26, indptr without B*K + 1 entries,
+    edge_index that is not int64 [2,E] (E < 2^31), tensors on different devices.  B, D, H, W = 0 and E = 0 launch
+    nothing.
+
+    Host behaviour is boundary_stats': one read of two int64 (the boundary voxel and pair counts) per chunk of volumes
+    (BOUNDARY_SCRATCH_CAP, a chunk whose pairs need more than the cap to sort halved and read again), RuntimeError under
+    CUDA graph capture before any device work.  Each row depends only on labels[b], values[b] and the entry."""
+    tensor("labels", labels, torch.int16, 4)
+    tensor("values", values, torch.float32, 5)
+    B, D, H, W = (int(v) for v in labels.shape)
+    if int(values.shape[0]) != B or tuple(int(v) for v in values.shape[2:]) != (D, H, W):
+        raise ValueError("values %s do not match labels %s" % (tuple(values.shape), (B, D, H, W)))
+    C = int(values.shape[1])
+    if C < 1:
+        raise ValueError("values needs at least one channel")
+    connectivity = check_connectivity_3d(connectivity)
+    K = check_K(K)
+    check_voxels(D, H, W, ": a boundary count could overflow int32")
+    P = voxel_pairs(D, H, W, connectivity)
+    if P > _INT_MAX:
+        raise ValueError("volumes of %dx%dx%d voxels have %d voxel pairs at connectivity %d, more than %d: a "
+                         "boundary count could overflow int32" % (D, H, W, P, connectivity, _INT_MAX))
+    edge_index, E = check_graph(graph, B, K)
+    if E > _INT_MAX:
+        raise ValueError("graph.edge_index has %d entries, more than %d: split the graph" % (E, _INT_MAX))
+    dev = cuda_device(labels, ("values", values), ("graph.indptr", graph.indptr), ("graph.edge_index", edge_index))
+    with torch.cuda.device(dev):
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("boundary_stats_3d reads its boundary pair count back to the host and cannot be captured "
+                               "in a CUDA graph")
+        if B == 0 or D == 0 or H == 0 or W == 0 or E == 0:  # no voxel pair: every row is absent
+            nan = float("nan")
+            return BoundaryStats(torch.full((E, C), nan, dtype=torch.float32, device=dev),
+                                 torch.full((E, C), nan, dtype=torch.float32, device=dev),
+                                 torch.full((E, C), nan, dtype=torch.float32, device=dev),
+                                 torch.zeros(E, dtype=torch.int32, device=dev))
+        out = BoundaryStats(*(torch.empty((E, C), dtype=torch.float32, device=dev) for _ in range(3)),
+                            torch.empty(E, dtype=torch.int32, device=dev))
+        lab = labels.contiguous()
+        val = values.detach().contiguous()
+        ei = edge_index.contiguous()
+        L = _lib.lib()
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        chunk = boundary3d_chunk(B, D, H, W, K, connectivity)
+        work = [(b0, min(chunk, B - b0)) for b0 in range(0, B, chunk)][::-1]
+        first = 1
+        while work:
+            b0, c = work.pop()
+            nbytes = int(L.fslic_b200_boundary3d_select_scratch_bytes(c, D, H, W, K, connectivity))
+            select = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            counts = torch.empty(2, dtype=torch.int64, device=dev)
+            _lib.check(L.fslic_b200_boundary3d_select_batch(dev.index, c, D, H, W, K, connectivity, lab[b0].data_ptr(),
+                                                            counts.data_ptr(), select.data_ptr(), nbytes, stream))
+            voxels, pairs = counts.tolist()  # the host wait: the boundary voxel and pair counts
+            sbytes = int(L.fslic_b200_boundary3d_stats_scratch_bytes(voxels, pairs, E))
+            if sbytes > BOUNDARY_SCRATCH_CAP and c > 1:  # too many pairs to sort at once: halve the chunk
+                work.extend([(b0 + c // 2, c - c // 2), (b0, c // 2)])
+                continue
+            scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
+            _lib.check(L.fslic_b200_boundary3d_stats_batch(
+                dev.index, c, D, H, W, K, C, connectivity, lab[b0].data_ptr(), val[b0].data_ptr(), voxels, pairs,
                 select.data_ptr(), nbytes, b0, B * K, E, ei[0].data_ptr(), ei[1].data_ptr(), first,
                 out.mean.data_ptr(), out.min.data_ptr(), out.max.data_ptr(), out.count.data_ptr(), scratch.data_ptr(),
                 sbytes, stream))

@@ -315,6 +315,19 @@ int fslic_b200_gt_scores_batch(int device, int batch, int H, int W, int K, int t
 /* d_out u8[B,H,W]: 1 where the right or lower neighbour exists and carries another label, else 0. */
 int fslic_b200_gt_boundaries_batch(int device, int batch, int H, int W, const uint16_t* d_labels, uint8_t* d_out,
                                    void* stream);
+/* The same over `batch` label volumes d_labels u16[B,D,H,W] and gt of that shape (DESIGN.md section 4.24);
+ * D * H * W <= 2^29.  The overlap fields are those of the [B, D*H, W] view.  A boundary voxel has a +x, +y or +z
+ * neighbour with another value (valid, for gt), and the window is the box |dz| <= rz, |dy| <= ry, |dx| <= rx (each
+ * 0..32) clipped to the volume.  Scratch bytes: as fslic_b200_gt_scores_scratch_bytes with H = D * H and two more
+ * bitmaps (5/8 byte per voxel in all); (size_t)-1 for bad arguments or when batch * D * H * W > 2^31 - 1 or
+ * batch > 2^17. */
+size_t fslic_b200_gt_scores3d_scratch_bytes(int batch, int D, int H, int W, int K);
+int fslic_b200_gt_scores3d_batch(int device, int batch, int D, int H, int W, int K, int rz, int ry, int rx, int dtype,
+                                 const void* d_gt, const uint16_t* d_labels, int has_ignore, long long ignore,
+                                 long long* d_out, void* d_scratch, size_t scratch_bytes, void* stream);
+/* d_out u8[B,D,H,W]: 1 where the +x, +y or +z neighbour exists and carries another label, else 0. */
+int fslic_b200_gt_boundaries3d_batch(int device, int batch, int D, int H, int W, const uint16_t* d_labels,
+                                     uint8_t* d_out, void* stream);
 
 /* Superpixel shapes (props.cuh; no counterpart in the reference) of `batch` label maps d_labels u16[B,H,W]; node
  * n = b*K + k is label k of image b, pixel (row y, column x) has coordinates (y, x).  A label outside [0, K) belongs to
@@ -411,6 +424,29 @@ int fslic_b200_boundary_stats_batch(int device, int batch, int H, int W, int K, 
                                     long long nodes, long long edges, const long long* d_src, const long long* d_dst,
                                     int first, float* d_mean, float* d_min, float* d_max, int32_t* d_count,
                                     void* d_scratch, size_t scratch_bytes, void* stream);
+/* The same over `batch` label volumes d_labels u16[B,D,H,W] and values d_values f32[B,C,D,H,W] (DESIGN.md section
+ * 4.24), with region_adjacency_3d's voxel pairs: each voxel (the anchor) with its forward neighbours (dz, dy, dx) of
+ * RAG3D_OFFSETS, the first 3 (connectivity 6), 9 (18) or 13 (26); the pair's ordinal is anchor * Ndir + d.  A volume
+ * has D * H * W <= 2^29 and at most 2^31 - 1 voxel pairs, a call at most 2^31 - 1 voxels.
+ * Scratch bytes of the select (the stats read it too): 6 per voxel and the larger temporary storage of the selection
+ * and the pair sum; 256 for no voxel; (size_t)-1 for bad arguments or volumes or calls over those limits. */
+size_t fslic_b200_boundary3d_select_scratch_bytes(int batch, int D, int H, int W, int K, int connectivity);
+/* d_counts int64[2]: the number of voxels with a boundary pair and the number of boundary pairs of the call. */
+int fslic_b200_boundary3d_select_batch(int device, int batch, int D, int H, int W, int K, int connectivity,
+                                       const uint16_t* d_labels, long long* d_counts, void* d_scratch,
+                                       size_t scratch_bytes, void* stream);
+/* Scratch bytes of the stats for `voxels` boundary voxels, `pairs` boundary pairs and `edges` graph entries: 4 per
+ * voxel, 34 per pair, 24 per entry and the largest temporary storage of the scan, the radix sorts and the selection;
+ * (size_t)-1 for a negative count, one above 2^31 - 1, or voxels > pairs > 13 * voxels. */
+size_t fslic_b200_boundary3d_stats_scratch_bytes(long long voxels, long long pairs, long long edges);
+/* After a select with the same batch, D, H, W, K, connectivity, d_labels and d_select_scratch, and `voxels` / `pairs`
+ * = its d_counts: the outputs of fslic_b200_boundary_stats_batch, with voxel pairs for pixel pairs. */
+int fslic_b200_boundary3d_stats_batch(int device, int batch, int D, int H, int W, int K, int C, int connectivity,
+                                      const uint16_t* d_labels, const float* d_values, long long voxels,
+                                      long long pairs, const void* d_select_scratch, size_t select_bytes,
+                                      long long image_base, long long nodes, long long edges, const long long* d_src,
+                                      const long long* d_dst, int first, float* d_mean, float* d_min, float* d_max,
+                                      int32_t* d_count, void* d_scratch, size_t scratch_bytes, void* stream);
 
 /* k-nearest-neighbour graphs over feature points (knn.cuh; the reference's get_knn_connectivity has no defined result)
  * of `batch` images of K points each, d_points f32[B,K,D], node n = b * K + i.  A node is a candidate when
